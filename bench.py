@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """bench.py — throughput of the multichannel demodulation hot path (BASELINE.json metric:
-"IQ Msamples/s through FFT+demod at 1/2/4/8 B200; % HBM roofline; vs CPU ref").
+"IQ Msamples/s through FFT+demod at 1/2/4/8 GPUs; % HBM roofline; vs CPU ref").
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg2|cfg1|cfg3|cfg3f|cfg4|cfg5] [--impl reference]
+                    [--dump-outputs DIR]
 
 A step = one pass of the hot path (K1 convert+window+DFT of the bins, K2 demodulation) over one batch of synthetic input:
 `batches_per_step` WAVE_BATCHes (default 64 x 125 ms = 8 s of signal) of every device of the workload, executed as
@@ -11,7 +12,7 @@ devices x 2.56 Msps U8, fft_size 2048, 8 AM channels each ("cfg2"); devices shar
 GPUs run N x 64 devices (scaling = "weak").
 
   value    device-timed (CUDA events on the engine's stream, max over ranks): IQ samples consumed / s, inputs resident in
-           HBM (the resident stream, 168 MB per run, is larger than the 126 MB L2: every run re-reads HBM).
+           HBM (the resident stream, 168 MB per run, is larger than the 50 MB L2: every run re-reads HBM).
   e2e      same metric through the public C ABI with HOST buffers: abg_push (H2D from pinned memory) + abg_run +
            abg_fetch_batches (results written by the GPU into pinned host slots, then copied to the caller's arrays) inside
            the timed region, software-pipelined by one run like any streaming caller; `pcie_frac` = achieved H2D rate /
@@ -27,6 +28,8 @@ GPUs run N x 64 devices (scaling = "weak").
            bounded sample of the workload: one pinned thread per device (multiple_demod_threads mode) and the reference's
            default single-thread round-robin, plus the cfg1 point.
 `--impl reference` times that CPU path alone (rank 0 only under torchrun) and prints the same line shape.
+`--dump-outputs DIR` writes what the last timed engine run computed (see dump_outputs) so that two builds can be compared
+output for output: the inputs are seeded, so the same arguments give the same inputs.
 """
 from __future__ import annotations
 
@@ -50,6 +53,8 @@ import numpy as np  # noqa: E402
 METRIC = "iq_msamples_per_s_fft_demod"
 UNIT = "Msamples/s"
 NB_RUN = 4  # WAVE_BATCHes per engine run (abg_options.max_batches_per_run)
+H100_SMS = 132
+DUMP_LIMIT_BYTES = 48 << 20
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -147,7 +152,7 @@ def cpu_description() -> dict:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -214,7 +219,7 @@ def measured_peaks():
             return json.load(open(path)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": 3350.0}, "fallback"
 
 
 def source_sha(*rel_paths) -> str:
@@ -389,6 +394,26 @@ def parity_spot(cfg, raws, nb, n_unique=4, relaxed=False, mixers=None, fft_mode=
     return out
 
 
+def dump_outputs(eng, out_dir: str, nb: int, B: int) -> dict:
+    """The last run's audio (channel_t.waveout, minus the first AGC_EXTRA samples, which the device already overwrote with
+    the next run's look-back) and squelch flags per batch, as float32 .npy; above DUMP_LIMIT_BYTES a seeded channel sample."""
+    from airband_b200 import config as cm
+    wout, axc = eng.run_outputs()
+    audio = wout[:, cm.AGC_EXTRA:nb * B]
+    G = audio.shape[0]
+    ch = np.arange(G)
+    if audio.nbytes > DUMP_LIMIT_BYTES:
+        keep = max(1, DUMP_LIMIT_BYTES // (audio.shape[1] * 4))
+        ch = np.sort(np.random.default_rng(0).choice(G, size=keep, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"waveout": np.ascontiguousarray(audio[ch], dtype=np.float32),
+              "axcindicate": np.ascontiguousarray(axc[:nb, ch], dtype=np.float32),
+              "channels": ch.astype(np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    return {"dir": out_dir, "channels": int(len(ch)), "of_channels": int(G), "bytes": int(sum(a.nbytes for a in arrays.values()))}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -402,6 +427,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the legs of the other BASELINE configs")
     ap.add_argument("--no-parity", action="store_true", help="skip the oracle parity spots of the legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the audio and squelch flags of the last timed engine run to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
     if args.batches_per_step % NB_RUN:
@@ -432,7 +459,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------------------------------ GPU arm
     numa = bind_to_gpu_numa(local_rank)   # before torch / CUDA allocate anything pinned
     import torch
     import torch.distributed as dist
@@ -543,6 +570,7 @@ def main():
         sampler.start()
         sampler.wait_first()
     elapsed_ms, launches, win = time_resident(eng, args.steps * runs_per_step, max(args.warmup, 3) * runs_per_step)
+    dumped = dump_outputs(eng, args.dump_outputs, NB_RUN, B) if (args.dump_outputs and rank == 0) else None
     clocks = None
     if rank == 0:
         windows = [win]
@@ -619,7 +647,7 @@ def main():
     alg_bytes = alg_bytes_per_run(cfg, NB_RUN)
     achieved = alg_bytes / (k1_ms * 1e-3) / 1e9
     kern = {1: "k1_fft_kernel (convert+window+full FFT+bin select, FP32)", 2: "k1_pruned_kernel (convert+window+output-pruned FFT, FP32)",
-            3: "k1_tc_kernel (raw bytes x window*twiddle digits as an int8 GEMM on tcgen05, S32 accumulators in TMEM)"}[path]
+            3: "k1_tc_kernel (raw bytes x window*twiddle digits as an int8 GEMM on wgmma, S32 accumulators in registers)"}[path]
     src_of = {1: "rtlsdr-airband_b200/csrc/k1_fft.cu", 2: "rtlsdr-airband_b200/csrc/k1_pruned.cu", 3: "rtlsdr-airband_b200/csrc/k1_tc.cu"}[path]
     sha = source_sha(src_of)
     traffic, issue = None, None
@@ -630,14 +658,14 @@ def main():
                 if cap.get("workload") == args.workload and cap.get("fft_path") == path and cap.get("source_sha") == sha:
                     traffic = cap.get("dram_bytes_per_launch")
                     if cap.get("warp_instructions_per_launch"):
-                        sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
+                        sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0
                         issue = {"warp_instructions_per_launch": cap["warp_instructions_per_launch"],
-                                 "issue_frac": cap["warp_instructions_per_launch"] / (148 * 4 * sm_mhz * 1e6 * k1_ms * 1e-3),
+                                 "issue_frac": cap["warp_instructions_per_launch"] / (H100_SMS * 4 * sm_mhz * 1e6 * k1_ms * 1e-3),
                                  "from": cap.get("file")}
         except Exception:
             pass
     roofline = {"bound": "hbm", "kernel": kern, "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-                "peak_source": peak_src + " (MEASURED_PEAKS.json hbm_gbs)" if peak_src == "measured" else "fallback 6650 GB/s",
+                "peak_source": peak_src + " (MEASURED_PEAKS.json hbm_gbs)" if peak_src == "measured" else "fallback: H100 SXM data sheet 3350 GB/s",
                 "traffic": traffic, "traffic_note": None if traffic else f"no ncu capture of this kernel source (sha {sha}) under profiles/k1_captures.json",
                 "alg_bytes_per_launch": alg_bytes, "k1_ms": k1_ms, "k2_ms": k2_ms, "k1_share_of_kernel_time": k1_ms / max(k1_ms + k2_ms, 1e-12),
                 "kernel_source_sha": sha, "issue": issue,
@@ -651,27 +679,29 @@ def main():
             k2sha = source_sha("rtlsdr-airband_b200/csrc/k2_demod.cu")
             for cap in json.load(open(tpath)):
                 if cap.get("workload") == args.workload and cap.get("fft_path") == "k2" and cap.get("source_sha") == k2sha and cap.get("warp_instructions_per_launch"):
-                    sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
+                    sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0
                     k2.update({"warp_instructions_per_launch": cap["warp_instructions_per_launch"],
                                "warp_instructions_per_sample": cap["warp_instructions_per_launch"] / k2["samples_per_launch"],
-                               "issue_frac": cap["warp_instructions_per_launch"] / (148 * 4 * sm_mhz * 1e6 * k2_ms * 1e-3), "from": cap.get("file")})
+                               "issue_frac": cap["warp_instructions_per_launch"] / (H100_SMS * 4 * sm_mhz * 1e6 * k2_ms * 1e-3), "from": cap.get("file")})
         except Exception:
             pass
     roofline["k2"] = k2
     if path == 3:
         C = max(len(dv.channels) for dv in cfg.devices)
-        nc = (4 * ((2 * C + 7) // 8 * 8) + 15) // 16 * 16
+        nc = (4 * ((2 * C + 7) // 8 * 8) + 31) // 32 * 32
         macs = frames_per_launch * 2 * N * nc
         roofline["tensor"] = {"int8_macs_per_launch": macs, "achieved_tops": 2 * macs / (k1_ms * 1e-3) / 1e12,
-                              "note": "executed tcgen05 kind::i8 work (frames x 2N bytes x columns); B200 int8 dense nominal 4500 TOPS"}
+                              "note": "executed wgmma int8 work (frames x 2N bytes x columns); H100 SXM int8 dense data-sheet figure 1979 TOPS"}
 
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": elapsed_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
             "data": "synthetic",
-            "config": dict(base_config, l2=(f"resident input {resident_bytes / 1e6:.0f} MB per engine run > 126 MB L2 (no flush needed)" if resident_bytes > 126e6
+            "config": dict(base_config, l2=(f"resident input {resident_bytes / 1e6:.0f} MB per engine run > 50 MB L2 (no flush needed)" if resident_bytes > 50e6
                                             else f"resident input {resident_bytes / 1e6:.0f} MB per engine run fits L2: value is L2-warm"),
                            k1_path=path),
             "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches), "roofline": roofline}
+    if dumped:
+        line["dumped_outputs"] = dumped
     eng.close()
 
     # ---- the other BASELINE configs ----
@@ -702,13 +732,13 @@ def main():
                        "realtime_floor_msps": sum(dv.sample_rate for dv in c.devices) / 1e6}
                 # issue-slot use of the two kernels, when profiles/k1_captures.json holds ncu captures of these exact sources
                 try:
-                    sm_hz = ((clocks or {}).get("sm_mhz") or 1965.0) * 1e6
+                    sm_hz = ((clocks or {}).get("sm_mhz") or 1980.0) * 1e6
                     src_k1 = {1: "rtlsdr-airband_b200/csrc/k1_fft.cu", 2: "rtlsdr-airband_b200/csrc/k1_pruned.cu", 3: "rtlsdr-airband_b200/csrc/k1_tc.cu"}[leg["k1_path"]]
                     want = {leg["k1_path"]: ("k1", source_sha(src_k1), a1), "k2": ("k2", source_sha("rtlsdr-airband_b200/csrc/k2_demod.cu"), a2)}
                     for cap in (json.load(open(tpath)) if os.path.exists(tpath) else []):
                         w_ = want.get(cap.get("fft_path"))
                         if cap.get("workload") == name and w_ and cap.get("source_sha") == w_[1] and cap.get("warp_instructions_per_launch"):
-                            leg[w_[0] + "_issue_frac"] = cap["warp_instructions_per_launch"] / (148 * 4 * sm_hz * w_[2] * 1e-3)
+                            leg[w_[0] + "_issue_frac"] = cap["warp_instructions_per_launch"] / (H100_SMS * 4 * sm_hz * w_[2] * 1e-3)
                             if w_[0] == "k1":
                                 leg["k1_dram_traffic_over_alg_bytes"] = cap["dram_bytes_per_launch"] / ab
                 except Exception:

@@ -1,5 +1,5 @@
 /*
- * airband_b200.h — C ABI of the B200 (sm_100a) multichannel demodulation engine.
+ * airband_b200.h — C ABI of the H100 (sm_90a) multichannel demodulation engine.
  *
  * Drop-in boundary for ONE path of RTLSDR-Airband: the body of demodulate()
  * (reference src/rtl_airband.cpp:286-672) — sample conversion + Blackman-Harris window + sliding FFT + per-channel
@@ -225,6 +225,9 @@ ABG_API int abg_mixer_device_buffers(abg_engine* e, float** dev_sums, int32_t** 
 /* Run conversion + window + FFT on one frame of `dev`'s format and return the full spectrum in natural bin order
  * (fftout[2*fft_size]); exercises the same kernel code as abg_run. */
 ABG_API int abg_debug_frame(abg_engine* e, int dev, const void* iq_frame, float* fftout);
+/* The most recent run's results as the device holds them (resident runs export nothing): wout float[Gp][P] channel-major
+ * audio ([0, AGC_EXTRA) is already the next run's look-back), axc[max_batches_per_run][Gp]; dims[4] = {G, Gp, P, nb}. */
+ABG_API int abg_debug_run_outputs(abg_engine* e, int32_t* dims, float* wout, unsigned char* axc);
 /* Feed |X[bin]| values straight into the demodulation state machine of one device (K1 skipped): wavein[C][n_batches *
  * WAVE_BATCH] becomes channel_t.wavein[AGC_EXTRA ...]; results are fetched as usual.  For the ports of the reference's own
  * Squelch / CTCSS unit tests (reference src/test_squelch.cpp:51-281, src/test_ctcss.cpp:122-155).  The device must not be
@@ -237,7 +240,7 @@ ABG_API int abg_debug_k1tc_trace(long long* out);
 ABG_API int abg_debug_k2_stats(unsigned long long* out);
 /* Host-only: plan and coefficient table of the tensor-core K1 (fft_mode 3) for one device, as abg_create builds them
  * (window * twiddle quantised to `digits` signed 8-bit digits, in the shared-memory image the MMA reads).
- * plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, tmem_cols, smem_bytes, halo, nacc}; tab == NULL queries the plan only. */
+ * plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups}; tab == NULL queries the plan only. */
 ABG_API int abg_debug_tc_table(int fft_size, int sfmt, int hop_bytes, float fullscale, int n_channels, const int32_t* bins, int digits,
                                int32_t* plan, signed char* tab, size_t tab_cap, long long* sq, double* cscale);
 

@@ -1,4 +1,4 @@
-// Internal layouts shared by the host engine and the two sm_100a kernels.
+// Internal layouts shared by the host engine and the two sm_90a kernels.
 //
 // Data layout in HBM (per engine = one GPU's share of devices[]):
 //   raw[d]            ring-format bytes of device d, linear, frames overlap in place (never expanded to float in HBM)
@@ -139,10 +139,10 @@ int abg_k1_tile_frames(int fft_size, int sfmt, int hop_bytes, int* tile_bytes_ca
 cudaError_t abg_launch_k1_pruned(const K1Launch& L, const float2* twn, int max_channels, cudaStream_t s);
 int abg_k1p_tile_frames(int fft_size, int sfmt, int hop_bytes, int max_channels, int* tile_bytes_cap);
 
-// tensor-core variant (k1_tc.cu): the bins' DFT as an integer GEMM on tcgen05 (8-bit formats, hop_bytes % 32 == 0)
+// tensor-core variant (k1_tc.cu): the bins' DFT as an integer GEMM on wgmma (8-bit formats, hop_bytes % 32 == 0)
 struct K1TcPlan {
     int eligible;
-    int K, HC, S, NC, ND, C2p, KBS, NSTB, tmem_cols, smem_bytes, halo, nacc;
+    int K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups;
     size_t table_bytes;
 };
 struct K1TcTables {

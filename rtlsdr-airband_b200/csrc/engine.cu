@@ -1,4 +1,4 @@
-// Host side of the B200 demodulation engine: configuration -> device tables and per-channel state, raw-sample
+// Host side of the demodulation engine: configuration -> device tables and per-channel state, raw-sample
 // ingest, run scheduling (K1 then K2 per run), result queueing, and the C ABI declared in include/airband_b200.h.
 //
 // Config-time arithmetic restated here (host, double/float exactly as the reference does it):
@@ -31,8 +31,8 @@ namespace {
 
 // Small host->device parameter uploads go through a KERNEL (payload passed by value), not cudaMemcpyAsync: a copy would
 // queue on the host->device copy engine behind whatever bulk ingest copies (abg_push of the NEXT run) are already
-// enqueued, and the run that needs these few hundred bytes would wait for megabytes of unrelated input (measured: ~1 ms
-// per step on the pipelined host path).  A launch is ordered only by its own stream.
+// enqueued, and the run that needs these few hundred bytes would wait for megabytes of unrelated input.  A launch is
+// ordered only by its own stream.
 struct UploadBlob {
     uint4 q[240];  // 3840 bytes: stays below the 4 KB kernel-parameter limit together with the other arguments
 };
@@ -277,7 +277,7 @@ struct Slot {
 
 struct abg_engine {
     int N = 0, W = 0, B = 0, fm_demod = 0, nbmax = 4, P = 0, G = 0, Gp = 0, fft_mode = 0;
-    int cuda_dev = 0, sm_count = 148, tc_digits = 4;
+    int cuda_dev = 0, sm_count = 132, tc_digits = 4;
     bool tc_auto = true;               // fft_mode 0 picks the tensor-core K1 for eligible groups (ABG_K1_TC_AUTO=0: FP32 kernels only)
     int32_t* tc_status = nullptr;      // pinned + mapped: the tensor-core K1 reports a stalled pipeline here (never hangs)
     int32_t* tc_status_dev = nullptr;
@@ -690,12 +690,12 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
         if (d.has_afc) e->any_afc = true;
     {
         // K2 is a sequential recurrence per channel.  One channel per warp (lane-parallel tiles, no divergence between
-        // channels in different squelch states) as long as that is at most 8 warps per SM sub-partition (measured on
-        // 4096 channels: K2 0.66 ms against 0.80 ms with 8 channels per warp); beyond that as few channels per warp as
-        // keeps the warp count near two per sub-partition.
+        // channels in different squelch states) as long as that is at most 8 warps per SM sub-partition; beyond that as
+        // few channels per warp as keeps the warp count near two per sub-partition.
+        const int subparts = 4 * e->sm_count;
         int lpw = 1;
-        if (e->G > 8 * 592)
-            while (lpw < 32 && (e->G + lpw - 1) / lpw > 2 * 592) lpw <<= 1;
+        if (e->G > 8 * subparts)
+            while (lpw < 32 && (e->G + lpw - 1) / lpw > 2 * subparts) lpw <<= 1;
         const char* env = getenv("ABG_K2_LPW");
         if (env && atoi(env) > 0) {
             lpw = 1;
@@ -957,7 +957,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
 extern "C" {
 
 const char* abg_last_error(void) { return g_err.c_str(); }
-const char* abg_version(void) { return "airband-b200 0.1 (sm_100a)"; }
+const char* abg_version(void) { return "airband-b200 0.1 (sm_90a)"; }
 
 int abg_create(const abg_config* cfg, const abg_options* opt, abg_engine** out) {
     if (!cfg || !out) return fail(ABG_EINVAL, "abg_create: null argument");
@@ -977,10 +977,10 @@ int abg_create(const abg_config* cfg, const abg_options* opt, abg_engine** out) 
         cudaGetDevice(&e->cuda_dev);
     }
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, e->cuda_dev) != cudaSuccess || prop.major < 10) {
-        int major = prop.major;
+    if (cudaGetDeviceProperties(&prop, e->cuda_dev) != cudaSuccess || prop.major != 9 || prop.minor != 0) {
+        const int major = prop.major, minor = prop.minor;
         delete e;
-        return fail(ABG_ENODEV, "CUDA device has compute capability %d.x; this library contains sm_100a code only", major);
+        return fail(ABG_ENODEV, "CUDA device has compute capability %d.%d; this library contains sm_90a code only", major, minor);
     }
     e->sm_count = prop.multiProcessorCount;
     int rc = build(e, cfg, opt);
@@ -1422,13 +1422,13 @@ int abg_mixer_device_buffers(abg_engine* e, float** dev_sums, int32_t** dev_flag
 }
 
 // Host-only (no device needed): the tensor-core K1's plan and coefficient table for one device, exactly as abg_create
-// builds them.  plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, tmem_cols, smem_bytes, halo, nacc}.  tab may be null to
+// builds them.  plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups}.  tab may be null to
 // query the plan; otherwise tab_cap >= K*NC bytes and sq has C2p entries.
 int abg_debug_tc_table(int fft_size, int sfmt, int hop_bytes, float fullscale, int n_channels, const int32_t* bins, int digits, int32_t* plan,
                        signed char* tab, size_t tab_cap, long long* sq, double* cscale) {
     K1TcPlan p;
     abg_k1tc_plan(fft_size, sfmt, hop_bytes, n_channels, digits, &p);
-    const int32_t v[13] = {p.eligible, p.K, p.HC, p.S, p.NC, p.ND, p.C2p, p.KBS, p.NSTB, p.tmem_cols, p.smem_bytes, p.halo, p.nacc};
+    const int32_t v[13] = {p.eligible, p.K, p.HC, p.S, p.NC, p.ND, p.C2p, p.KBS, p.NSTB, p.acc_regs, p.smem_bytes, p.halo, p.consumer_warpgroups};
     if (plan) memcpy(plan, v, sizeof(v));
     if (!p.eligible) return fail(ABG_EINVAL, "abg_debug_tc_table: configuration not eligible for the tensor-core K1");
     if (!tab) return ABG_OK;
@@ -1473,6 +1473,19 @@ int abg_debug_inject_wavein(abg_engine* e, int dev, int n_batches, const float* 
 // abg_create); out[256][4 roles][16 tiles][4 events]
 int abg_debug_k2_stats(unsigned long long* out) { return abg_k2_stats_dump(out) == 0 ? ABG_OK : fail(ABG_EINVAL, "no counters: not an ABG_K2_STATS build (make stats)"); }
 int abg_debug_k1tc_trace(long long* out) { return abg_k1tc_trace_dump(out) == 0 ? ABG_OK : fail(ABG_EINVAL, "no trace: ABG_K1_TC_TRACE was not set"); }
+
+// see airband_b200.h: the most recent run's wout[Gp][P] and axc[max_batches_per_run][Gp] as the device holds them
+int abg_debug_run_outputs(abg_engine* e, int32_t* dims, float* wout, unsigned char* axc) {
+    if (dims) {
+        dims[0] = e->G; dims[1] = e->Gp; dims[2] = e->P; dims[3] = e->nbmax;
+    }
+    if (!wout && !axc) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaDeviceSynchronize());
+    if (wout) CU(cudaMemcpy(wout, e->wout.p, sizeof(float) * (size_t)e->Gp * e->P, cudaMemcpyDeviceToHost));
+    if (axc) CU(cudaMemcpy(axc, e->axc.p, (size_t)e->nbmax * e->Gp, cudaMemcpyDeviceToHost));
+    return ABG_OK;
+}
 
 int abg_debug_frame(abg_engine* e, int dev, const void* iq_frame, float* fftout) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_debug_frame: device %d out of range", dev);

@@ -1,4 +1,4 @@
-// K1 — fused sample conversion + Blackman-Harris window + batched FFT + per-channel bin extraction (sm_100a).
+// K1 — fused sample conversion + Blackman-Harris window + batched FFT + per-channel bin extraction (sm_90a).
 //
 // Replaces, for every frame of every device, the reference's three hot loops
 //   convert+window   reference src/rtl_airband.cpp:402-455

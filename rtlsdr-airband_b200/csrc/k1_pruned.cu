@@ -1,5 +1,5 @@
 // K1 (output-pruned) — fused sample conversion + window + FFT + per-channel bin extraction, computing ONLY the
-// configured bins in the last pass (sm_100a).  Same inputs, same outputs as k1_fft.cu; replaces the same reference
+// configured bins in the last pass (sm_90a).  Same inputs, same outputs as k1_fft.cu; replaces the same reference
 // code (reference src/rtl_airband.cpp:402-455 convert+window, :460 fftwf_execute, :483-489 bin extraction).
 //
 // The reference runs a full N-point FFT per frame and then reads C of the N bins (C = channels of the device,
@@ -163,8 +163,8 @@ __global__ void __launch_bounds__(PR_WARPS * 32) k1_pruned_kernel(const PrArgs a
     mbar_wait0(mbar);
 
     float* part = s_part + warp * (2 * CM * PR_PAD);
-    // (register-resident accumulators across the groups for devices with few channels were measured SLOWER on B200:
-    // 0.618 vs 0.541 ms on cfg2, 102 registers and a much larger unrolled body; partial sums go through shared memory)
+    // (partial sums go through shared memory: register-resident accumulators across the groups for devices with few
+    // channels need ~100 registers and a much larger unrolled body)
     const float* __restrict__ wsc = a.wsc;
     const int iters = (nf + PR_WARPS - 1) / PR_WARPS;
     for (int it = 0; it < iters; ++it) {

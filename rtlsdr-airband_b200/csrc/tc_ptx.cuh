@@ -1,14 +1,12 @@
-// Inline-PTX building blocks of the tensor-core K1 (k1_tc.cu) for sm_100a: mbarrier, cp.async / bulk copies,
-// tcgen05 (TMEM allocation, UMMA shared-memory / instruction descriptors, kind::i8 MMA, commit, TMEM loads).
+// Inline-PTX building blocks of the tensor-core K1 (k1_tc.cu) for sm_90a: mbarrier, cp.async / bulk copies, and the
+// warpgroup MMA (wgmma.mma_async, 8-bit integer operands from shared memory, S32 accumulators in registers).
 //
-// Descriptor encodings follow the PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor" tables:
+// Descriptor encoding follows the PTX ISA "Matrix Descriptor Format" table of the warpgroup MMA:
 //   shared-memory descriptor (64 bit): [0,14) start address >> 4 | [16,30) leading byte offset >> 4 |
-//       [32,46) stride byte offset >> 4 | [46,48) version = 1 | [49,52) base offset | [61,64) swizzle (0 = none)
+//       [32,46) stride byte offset >> 4 | [49,52) base offset | [62,64) swizzle mode (0 = none)
 //   K-major operand without swizzle ("interleaved" canonical layout): 8 rows x 16 bytes form one 128-byte core
 //   matrix; LBO = byte distance between the two 16-byte K chunks of one MMA (K = 32 bytes for 8-bit types),
-//   SBO = byte distance between consecutive 8-row groups along M (or N).
-//   instruction descriptor (32 bit): [4,6) D format (2 = S32) | [7,10) A format (0 = U8, 1 = S8) | [10,13) B format |
-//       [15] A major (0 = K) | [16] B major (0 = K) | [17,23) N >> 3 | [24,29) M >> 4
+//   SBO = byte distance between consecutive 8-row groups along M (or N).  8-bit operands must be K-major.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -119,7 +117,7 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-// generic-proxy writes (st.shared, cp.async) -> visible to the async proxy (tcgen05.mma operand reads, bulk copies)
+// generic-proxy writes (st.shared, cp.async) -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // TMA bulk copy global -> shared, completion counted in bytes on an mbarrier
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
@@ -128,86 +126,69 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                  : "memory");
 }
 
-// ---- tcgen05 --------------------------------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem) {  // whole warp; NCOLS a power of two in [32, 512]
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "n"(NCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp (the one that allocated)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
+// ---- wgmma ----------------------------------------------------------------------------------------------------------
 __host__ __device__ constexpr uint64_t smem_desc_noswizzle(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) |
-           (1ull << 46);
+    return (uint64_t)((addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32);
 }
-__host__ __device__ constexpr uint32_t idesc_i8(int m, int n, int a_signed, int b_signed) {
-    return (2u << 4) | ((uint32_t)(a_signed ? 1 : 0) << 7) | ((uint32_t)(b_signed ? 1 : 0) << 10) | ((uint32_t)(n >> 3) << 17) |
-           ((uint32_t)(m >> 4) << 24);
+// accumulator registers may be written by wgmma.mma_async only after this (every warp of the warpgroup)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of an accumulator register across the asynchronous MMAs that own it
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(uint32_t (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]^T, 8-bit integer operands, S32 accumulator; issued by ONE thread
-__device__ __forceinline__ void mma_i8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-        :
-        : "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// same, descriptors passed as 32-bit halves (the low word carries the start address and is the only part that changes
-// from one K step to the next: no 64-bit arithmetic in the issue loop)
-__device__ __forceinline__ void mma_i8_split(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], da, db, %5, p;\n\t}"
-        :
-        : "r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// predicated forms (issue != 0 on exactly one lane of the warp): no divergent branch around the instruction, so the loop that
-// computes the operands stays warp-uniform for the compiler
-__device__ __forceinline__ void mma_i8_split_if(uint32_t issue, uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                                uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "setp.ne.b32 q, %7, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::i8 [%0], da, db, %5, p;\n\t}"
-        :
-        : "r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate), "r"(issue)
-        : "memory");
-}
-__device__ __forceinline__ void mma_commit_if(uint32_t issue, uint32_t bar) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "setp.ne.b32 q, %1, 0;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-        :
-        : "r"(bar), "r"(issue)
-        : "memory");
-}
-// mbarrier arrive once every MMA issued so far by this thread has completed (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 32 bit, 8 consecutive columns: thread t of warp w reads TMEM lane 32*(w%4)+t
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// D[64 x N] (+)= A[64 x 32] * B[N x 32]^T for one warpgroup, both operands K-major in shared memory, A unsigned or signed
+// 8-bit (a_signed, warp-uniform), B signed 8-bit, S32 accumulators: thread t of the warpgroup holds d[4j + 2h + e] =
+// D[16 (t / 32) + (t % 32) / 4 + 8h][8j + 2 (t % 4) + e].  acc == 0 overwrites D.
+template <int N>
+struct WgmmaI8;
+// accumulator operand lists, 8 registers at a time, and the matching register strings, 16 at a time
+#define ABG_D8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
+#define ABG_D16 ABG_D8(0), ABG_D8(8)
+#define ABG_S16 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define ABG_D32 ABG_D16, ABG_D8(16), ABG_D8(24)
+#define ABG_S32 ABG_S16 ", %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define ABG_D48 ABG_D32, ABG_D8(32), ABG_D8(40)
+#define ABG_S48 ABG_S32 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define ABG_D64 ABG_D48, ABG_D8(48), ABG_D8(56)
+#define ABG_S64 ABG_S48 ", %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define ABG_D80 ABG_D64, ABG_D8(64), ABG_D8(72)
+#define ABG_S80 ABG_S64 ", %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+#define ABG_D96 ABG_D80, ABG_D8(80), ABG_D8(88)
+#define ABG_S96 ABG_S80 ", %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define ABG_D112 ABG_D96, ABG_D8(96), ABG_D8(104)
+#define ABG_S112 ABG_S96 ", %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111"
+#define ABG_D128 ABG_D112, ABG_D8(112), ABG_D8(120)
+#define ABG_S128 ABG_S112 ", %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+#define ABG_WGMMA_I8(N, R, P, A, B) \
+    template <> \
+    struct WgmmaI8<N> { \
+        static __device__ __forceinline__ void mma(uint32_t (&d)[R], uint64_t a, uint64_t b, uint32_t acc, uint32_t a_signed) { \
+            if (a_signed) \
+                asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\t" \
+                             "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32.s8.s8 {" ABG_S##R "}, " A ", " B ", p;\n\t}" \
+                             : ABG_D##R \
+                             : "l"(a), "l"(b), "r"(acc)); \
+            else \
+                asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\t" \
+                             "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32.u8.s8 {" ABG_S##R "}, " A ", " B ", p;\n\t}" \
+                             : ABG_D##R \
+                             : "l"(a), "l"(b), "r"(acc)); \
+        } \
+    };
+ABG_WGMMA_I8(32, 16, "%18", "%16", "%17")
+ABG_WGMMA_I8(64, 32, "%34", "%32", "%33")
+ABG_WGMMA_I8(96, 48, "%50", "%48", "%49")
+ABG_WGMMA_I8(128, 64, "%66", "%64", "%65")
+ABG_WGMMA_I8(160, 80, "%82", "%80", "%81")
+ABG_WGMMA_I8(192, 96, "%98", "%96", "%97")
+ABG_WGMMA_I8(224, 112, "%114", "%112", "%113")
+ABG_WGMMA_I8(256, 128, "%130", "%128", "%129")
+#undef ABG_WGMMA_I8
 
 }  // namespace tc

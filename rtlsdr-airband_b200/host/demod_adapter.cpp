@@ -1,4 +1,4 @@
-// demodulate_b200(): the reference's demod thread function re-expressed over the C ABI of the B200 engine.
+// demodulate_b200(): the reference's demod thread function re-expressed over the C ABI of the GPU engine.
 // Same contract as demodulate() (reference src/rtl_airband.cpp:286-672): it owns devices[device_start..device_end),
 // consumes each input ring under the reference's locking discipline (:370-375, bufs advanced without the lock, :669),
 // follows the input state machine (:377-391, including disable_device_outputs() for a dead receiver), delivers finished
@@ -197,7 +197,7 @@ extern "C" void* demodulate_b200(void* params) {
     opt.input_capacity_batches = opt.max_batches_per_run + 2;
     abg_engine* eng = nullptr;
     if (abg_create(&cfg, &opt, &eng) != ABG_OK) {
-        fatal("Unable to start the B200 demodulation engine");
+        fatal("Unable to start the GPU demodulation engine");
         return NULL;
     }
     // ---- ingest bridge: pin the input rings in place so that abg_push is asynchronous DMA straight out of the ring the
@@ -407,6 +407,10 @@ extern "C" void* demodulate_b200(void* params) {
         if (idle) {
             bool waiting = false;  // batches held back only because the output thread has not consumed the previous one
             for (int i = 0; i < nd; i++) waiting = waiting || abg_batches_ready(eng, i) > 0;
+            // (deliver_mixers does not look further while the output thread has not taken a mixer's last batch: more may be
+            // queued behind it)
+            if (g_b200.wait_for_consumer)
+                for (const auto& gm : g_gpu_mixers) waiting = waiting || gm.mixer->channel.state == CH_READY;
             if (waiting) idle = false;
             usleep(waiting ? 200 : 10 * 1000);  // SLEEP(10), :398
         }

@@ -362,7 +362,7 @@ ABG_API int abh_run_pattern(void* hp, const unsigned char* const* blocks, const 
     if (!proto) return -3;
     for (int i = 0; i < D; i++) {
         input_t& in = h->inputs[i];
-        dd[i] = {blocks[i], block_bytes[i], repeat, speedup};
+        dd[i] = {blocks[i], block_bytes[i], repeat, speedup, 0};
         in.dev_data = &dd[i];
         in.init = proto->init;
         in.run_rx_thread = proto->run_rx_thread;
@@ -393,7 +393,8 @@ static int run_with_inputs(Harness* h, std::vector<pthread_t>& fth, int timeout_
     Consumer cons = {h, 0};
     pthread_create(&cth, NULL, consumer_thread, &cons);
     pthread_create(&dth, NULL, demodulate_b200, &dp);
-    // finished when every feeder has ended, every ring is (nearly) empty and nothing new arrived for a while
+    // finished when every feeder has ended, every ring is (nearly) empty and nothing new arrived for a while: longer than
+    // the second demodulate_b200 waits for a stalled mixer input before it sums without it
     int idle_ms = 0, last_total = -1, waited_ms = 0;
     while (!g_b200.do_exit && waited_ms < timeout_s * 1000) {
         usleep(20 * 1000);
@@ -402,12 +403,13 @@ static int run_with_inputs(Harness* h, std::vector<pthread_t>& fth, int timeout_
         for (int i = 0; i < D; i++) fed = fed && (h->inputs[i].state == INPUT_FAILED || h->inputs[i].state == INPUT_DISABLED);
         int total = 0;
         for (int i = 0; i < D; i++) total += h->n_batches[i];
+        for (size_t m = 0; m < h->mixers.size(); m++) total += h->n_mix_batches[m];
         if (fed && total == last_total)
             idle_ms += 20;
         else
             idle_ms = 0;
         last_total = total;
-        if (fed && idle_ms >= 400) break;
+        if (fed && idle_ms >= 1500) break;
     }
     const bool timed_out = waited_ms >= timeout_s * 1000;
     g_b200.do_exit = 1;
@@ -435,7 +437,7 @@ ABG_API long abh_pattern_selftest(int sfmt, int sample_rate, size_t fft_size, co
     in->bytes_per_sample = sfmt == ABG_SFMT_S16 ? 2 : (sfmt == ABG_SFMT_F32 ? 4 : 1);
     in->sample_rate = sample_rate;
     pattern_dev_data_t* dd = (pattern_dev_data_t*)in->dev_data;
-    *dd = {block, block_len, repeat, speedup};
+    *dd = {block, block_len, repeat, speedup, 0};
     const size_t bpc = 2 * (size_t)in->bytes_per_sample, tail = bpc * fft_size;
     in->buf_size = 256 * 1024;  // a small ring so that it wraps many times
     in->buf_size -= in->buf_size % bpc;
@@ -453,6 +455,7 @@ ABG_API long abh_pattern_selftest(int sfmt, int sample_rate, size_t fft_size, co
     size_t pos = 0;
     const size_t total = block_len * (size_t)repeat;
     int idle_ms = 0;
+    bool lapped = false;
     while (idle_ms < 2000) {
         size_t available;
         pthread_mutex_lock(&in->buffer_lock);
@@ -465,11 +468,18 @@ ABG_API long abh_pattern_selftest(int sfmt, int sample_rate, size_t fft_size, co
             continue;
         }
         idle_ms = 0;
-        if (in->overflow_count == 0) {  // after an overflow the byte positions no longer line up: only count from then on
+        if (!lapped) {  // after an overflow the byte positions no longer line up: only count until then
+            long mismatches = 0;
             for (size_t k = 0; k < available; k++) {
                 const unsigned char got = in->buffer[(in->bufs + k) % in->buf_size];
-                if (got != block[(pos + k) % block_len]) bad++;
+                if (got != block[(pos + k) % block_len]) mismatches++;
             }
+            // valid only if the producer has not yet written stream position pos + buf_size (overflow_count misses laps
+            // that wrap past the ring end, as in the reference)
+            pthread_mutex_lock(&in->buffer_lock);
+            lapped = in->overflow_count > 0 || __atomic_load_n(&dd->queued, __ATOMIC_SEQ_CST) > pos + in->buf_size;
+            pthread_mutex_unlock(&in->buffer_lock);
+            if (!lapped) bad += mismatches;
         }
         pos += available;
         in->bufs = (in->bufs + available) % in->buf_size;  // not under the lock, like rtl_airband.cpp:669
@@ -479,7 +489,7 @@ ABG_API long abh_pattern_selftest(int sfmt, int sample_rate, size_t fft_size, co
     pthread_join(in->rx_thread, NULL);
     if (consumed) *consumed = pos;
     if (overflows) *overflows = in->overflow_count;
-    if (in->overflow_count == 0 && pos != total) bad += 1000000;
+    if (!lapped && pos != total) bad += 1000000;
     pthread_mutex_destroy(&in->buffer_lock);
     free(in->dev_data);
     free(in);

@@ -1,4 +1,4 @@
-"""Configuration records for the B200 demodulation path and their C layout.
+"""Configuration records for the GPU demodulation path and their C layout.
 
 The C structs are declared in include/airband_b200.h (abg_channel_cfg / abg_device_cfg / abg_config); they
 carry exactly what the reference's demodulate() reads from device_t / channel_t / freq_t / input_t

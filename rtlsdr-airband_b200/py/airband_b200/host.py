@@ -1,5 +1,5 @@
 """ctypes driver of the C++ host adapter test harness (rtlsdr-airband_b200/host): input rings + demodulate_b200() +
-an output-thread stand-in, i.e. the reference's thread structure around the B200 engine."""
+an output-thread stand-in, i.e. the reference's thread structure around the GPU engine."""
 from __future__ import annotations
 
 import ctypes as C

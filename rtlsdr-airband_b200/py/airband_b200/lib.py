@@ -1,6 +1,6 @@
 """ctypes binding of the product: rtlsdr-airband_b200/libairband_b200.so (C ABI in include/airband_b200.h).
 
-There is no fallback of any kind here: if the shared library is missing, or no sm_100 device is present,
+There is no fallback of any kind here: if the shared library is missing, or no sm_90 (H100) device is present,
 construction raises.  (The CPU oracle under oracle/ is test infrastructure and is never imported from here.)
 """
 from __future__ import annotations
@@ -23,6 +23,7 @@ SYMBOLS = [
     "abg_batches_available", "abg_run", "abg_sync", "abg_join", "abg_batches_ready", "abg_fetch_batch", "abg_fetch_batches", "abg_get_stats", "abg_set_bin",
     "abg_resident_load", "abg_run_resident", "abg_set_stream", "abg_launch_count", "abg_mixers_configure",
     "abg_fetch_mixer_batch", "abg_mixer_device_buffers", "abg_debug_frame", "abg_last_run_times", "abg_debug_timeline", "abg_scan_configure", "abg_scan_select", "abg_host_register", "abg_host_unregister", "abg_ingest_sync", "abg_fft_path", "abg_debug_tc_table", "abg_debug_inject_wavein", "abg_debug_k1tc_trace", "abg_debug_k2_stats",
+    "abg_debug_run_outputs",
 ]
 
 
@@ -83,6 +84,7 @@ def load():
     L.abg_fetch_mixer_batch.restype, L.abg_fetch_mixer_batch.argtypes = i, [vp, i, vp, vp, C.POINTER(C.c_int)]
     L.abg_mixer_device_buffers.restype, L.abg_mixer_device_buffers.argtypes = i, [vp, C.POINTER(vp), C.POINTER(vp)]
     L.abg_debug_frame.restype, L.abg_debug_frame.argtypes = i, [vp, i, vp, vp]
+    L.abg_debug_run_outputs.restype, L.abg_debug_run_outputs.argtypes = i, [vp, vp, vp, vp]
     L.abg_last_run_times.restype, L.abg_last_run_times.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_host_register.restype, L.abg_host_register.argtypes = i, [vp, C.c_size_t]
     L.abg_host_unregister.restype, L.abg_host_unregister.argtypes = i, [vp]
@@ -212,6 +214,16 @@ class Engine:
     def run_resident(self, n_batches: int) -> int:
         return self._chk(self.L.abg_run_resident(self.h, n_batches))
 
+    def run_outputs(self):
+        """(wout[G, P], axc[max_batches_per_run, G]) of the most recent run, resident runs included (abg_debug_run_outputs)."""
+        dims = np.zeros(4, np.int32)
+        self._chk(self.L.abg_debug_run_outputs(self.h, _ptr(dims), None, None))
+        G, Gp, P, nb = (int(x) for x in dims)
+        wout = np.empty((Gp, P), np.float32)
+        axc = np.empty((nb, Gp), np.uint8)
+        self._chk(self.L.abg_debug_run_outputs(self.h, _ptr(dims), _ptr(wout), _ptr(axc)))
+        return wout[:G], axc[:, :G]
+
     def set_stream(self, cuda_stream_ptr: int) -> None:
         self._chk(self.L.abg_set_stream(self.h, C.c_void_p(cuda_stream_ptr)))
 
@@ -280,7 +292,7 @@ class Engine:
         return out.view(np.complex64)
 
 
-TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "tmem_cols", "smem_bytes", "halo", "nacc")
+TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "acc_regs", "smem_bytes", "halo", "consumer_warpgroups")
 
 
 def tc_table(fft_size: int, sfmt: int, hop_bytes: int, bins: Sequence[int], digits: int = 4, fullscale: float = 1.0):

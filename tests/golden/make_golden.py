@@ -1,13 +1,11 @@
-#!/usr/bin/env python
-"""Generates tests/golden/*.npz.  Run in the authoring container, where /root/reference exists:
+"""Generates tests/golden/*.npz from oracle/_ref (`make -C oracle REF=<reference checkout>`):
 
     python tests/golden/make_golden.py
 
-For every case in tests/cases.py listed in GOLDEN it stores the exact raw I/Q bytes fed in and the outputs of
+For every case in tests/cases.py it stores the SHA-256 of the raw I/Q bytes fed in and the outputs of
 oracle/_ref/libairband_ref.so — i.e. the reference's OWN squelch.cpp / ctcss.cpp / filters.cpp (compiled in place
-from /root/reference/src by oracle/Makefile) behind the restated demodulate() loop and the FP32 FFT stand-in.
-(The reference's main translation unit cannot be built here: lame/shout/libconfig++/fftw3 are absent.)
-The fixtures travel to the GPU box, where /root/reference does not exist."""
+by oracle/Makefile) behind the restated demodulate() loop and the FP32 FFT stand-in, and in ref_leaf.npz the SHA-256
+of the reference leaf classes' outputs that test_oracle_leaf_vs_ref.py and test_oracle_scan.py compare with."""
 import os
 import sys
 
@@ -18,10 +16,16 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 for p in (os.path.join(ROOT, "tests"), os.path.join(ROOT, "oracle"), os.path.join(ROOT, "rtlsdr-airband_b200", "py")):
     sys.path.insert(0, p)
 
+import hashlib  # noqa: E402
+
 import oracle_py as op  # noqa: E402
 from cases import CASES  # noqa: E402
 
-GOLDEN = ["am_u8", "nfm_s16", "am_bw_f32", "s8_two_devices"]
+GOLDEN = list(CASES)
+
+
+def sha256(a: np.ndarray) -> np.ndarray:
+    return np.frombuffer(hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest(), np.uint8)
 
 
 def main():
@@ -31,7 +35,7 @@ def main():
         res, o = op.run_oracle(cfg, raws, "ref")
         out = {}
         for d, (wo, iq, ax) in enumerate(res):
-            out[f"raw{d}"] = raws[d]
+            out[f"raw{d}_sha256"] = sha256(raws[d])
             out[f"waveout{d}"] = wo
             out[f"iq_out{d}"] = iq
             out[f"axc{d}"] = ax
@@ -43,6 +47,15 @@ def main():
         path = os.path.join(HERE, name + ".npz")
         np.savez_compressed(path, **out)
         print(name, os.path.getsize(path), "bytes")
+    import test_oracle_leaf_vs_ref as leaf
+    import test_oracle_scan as scan
+    ref = {}
+    ref.update(leaf.reference_outputs())
+    ref.update(scan.reference_outputs())
+    ref = {k: sha256(v) for k, v in ref.items()}
+    path = os.path.join(HERE, "ref_leaf.npz")
+    np.savez_compressed(path, **ref)
+    print("ref_leaf", os.path.getsize(path), "bytes")
 
 
 if __name__ == "__main__":

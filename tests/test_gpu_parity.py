@@ -2,6 +2,7 @@
 seeded inputs, and against the committed golden fixtures.
 Gate (BASELINE.md §3): per audio sample |gpu - oracle| <= 1e-4 * max(1, |gpu|, |oracle|) — float32 path, tolerance
 1e-4 as north_star states — plus identical squelch decisions (axcindicate per batch, open/flap/CTCSS counters)."""
+import hashlib
 import os
 
 import numpy as np
@@ -52,8 +53,9 @@ def test_case_matches_oracle(name, fft_mode):
 @pytest.mark.parametrize("name", ["am_u8", "nfm_s16", "am_bw_f32", "s8_two_devices"])
 def test_case_matches_golden_fixture(name):
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", name + ".npz"))
-    cfg, _ = CASES[name]()
-    raws = [g[f"raw{d}"] for d in range(len(cfg.devices))]
+    cfg, raws = CASES[name]()
+    for d, r in enumerate(raws):  # the bytes the fixture was made from
+        assert hashlib.sha256(np.ascontiguousarray(r).tobytes()).digest() == g[f"raw{d}_sha256"].tobytes()
     gres, geng = lib.demodulate_all(cfg, raws)
     for d, (gw, gi, ga) in enumerate(gres):
         assert np.array_equal(ga, g[f"axc{d}"])

@@ -1,5 +1,5 @@
 """GPU parity tests of the tensor-core K1 (fft_mode 3, rtlsdr-airband_b200/csrc/k1_tc.cu): the configured bins' DFT as an
-integer GEMM on tcgen05 with the raw bytes as the A operand.  Same gate as every other path (BASELINE.md §3): audio
+integer GEMM on wgmma with the raw bytes as the A operand.  Same gate as every other path (BASELINE.md §3): audio
 within 1e-4 of the CPU oracle, identical squelch decisions and counters; plus the properties that do not need the oracle
 at BASELINE sizes (twin devices bit-identical, agreement with the FP32 kernels, batching invariance)."""
 import numpy as np

@@ -1,12 +1,17 @@
 """Scan mode of the oracle (reference: freqlist[] / freq_idx, src/rtl_airband.h:223-233,250-252; controller_thread
 src/rtl_airband.cpp:101-139; fparms picked per batch, :498): every frequency-list entry owns its Squelch, filters,
 AGC and counters, the channel keeps its waveform history."""
+import hashlib
+import os
+
 import numpy as np
 import pytest
 
 import oracle_py as op
 from airband_b200 import config as cm
 from airband_b200 import workloads as wl
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_leaf.npz")
 
 
 def _setup():
@@ -77,11 +82,27 @@ def test_entries_keep_their_own_state():
     assert not np.array_equal(w_, w2)
 
 
-@pytest.mark.skipif(not op.available("ref"), reason="oracle/_ref not built")
-def test_scan_restated_equals_reference_leaf():
+def _scan_case(variant):
     cfg, freqs = _setup()
     visits = [0, 1, 2, 1, 0, 2, 2, 0]
     raw = wl.synth_iq(cfg, 0, wl.samples_for_batches(cfg, 0, 4 * len(visits)), key_on_s=1.2, key_off_s=0.2, amplitude=0.2)
-    a, xa, sa = _run(cfg, freqs, visits, raw, "restated")
-    b, xb, sb = _run(cfg, freqs, visits, raw, "ref")
-    assert np.array_equal(a.view(np.uint32), b.view(np.uint32)) and np.array_equal(xa, xb) and sa == sb
+    return _run(cfg, freqs, visits, raw, variant)
+
+
+def reference_outputs() -> dict:
+    """The reference leaf classes' result of the scan case (tests/golden/make_golden.py stores its SHA-256)."""
+    b, xb, sb = _scan_case("ref")
+    return {"scan_waveout": b, "scan_axc": xb, "scan_stats": np.array(sb, np.int64)}
+
+
+def test_scan_restated_equals_reference_leaf():
+    """Bit for bit against the reference leaf classes' result: live from oracle/_ref when it is built, and always the
+    SHA-256 of that result stored in tests/golden/ref_leaf.npz."""
+    a, xa, sa = _scan_case("restated")
+    got = {"scan_waveout": a, "scan_axc": xa, "scan_stats": np.array(sa, np.int64)}
+    if op.available("ref"):
+        b, xb, sb = _scan_case("ref")
+        assert np.array_equal(a.view(np.uint32), b.view(np.uint32)) and np.array_equal(xa, xb) and sa == sb
+    g = np.load(GOLDEN)
+    for k, v in got.items():
+        assert np.array_equal(np.frombuffer(hashlib.sha256(np.ascontiguousarray(v).tobytes()).digest(), np.uint8), g[k]), k

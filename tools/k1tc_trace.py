@@ -29,8 +29,8 @@ buf = np.zeros(256 * 4 * 16 * 4, np.int64)
 assert eng.L.abg_debug_k1tc_trace(buf.ctypes.data_as(C.c_void_p)) == 0
 t = buf.reshape(256, 4, 16, 4)[cta]
 t0 = t[t > 0].min()
-names = {0: ("producer", ["info seen", "empty_a ok", "copies issued", "arrived full_a"]), 1: ("epilogue", ["info seen", "tmem_full ok", "done", "-"]),
-         2: ("loader", ["tile start", "tile B issued", "-", "-"]), 3: ("mma", ["info seen", "full_a ok", "tmem_empty ok", "tile committed"])}
+names = {0: ("producer", ["info seen", "empty_a ok", "copies issued", "arrived full_a"]), 1: ("epilogue", ["-", "accumulators ready", "done", "-"]),
+         2: ("loader", ["tile start", "tile B issued", "-", "-"]), 3: ("mma", ["info seen", "full_a ok", "-", "-"])}
 for tile in range(6):
     print(f"tile {tile}")
     for role in range(4):

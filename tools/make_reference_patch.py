@@ -28,7 +28,7 @@ def sub_once(text, old, new, what):
 
 
 def edit_header(t):
-    t = sub_once(t, '#include "squelch.h"\n', '#include "squelch.h"\n\n#ifdef WITH_B200\n#include "airband_b200.h"       // C ABI of the B200 demodulation engine\n'
+    t = sub_once(t, '#include "squelch.h"\n', '#include "squelch.h"\n\n#ifdef WITH_B200\n#include "airband_b200.h"       // C ABI of the GPU demodulation engine\n'
                  '#include "airband_b200_host.h"  // b200_freq_cfg, b200_freq_stats\n#endif /* WITH_B200 */\n', "engine headers")
     t = sub_once(t, "    enum modulations modulation;\n};\n", "    enum modulations modulation;\n#ifdef WITH_B200\n    b200_freq_cfg b200_cfg;      // what config.cpp handed to squelch / notch_filter / lowpass_filter\n"
                  "    b200_freq_stats b200_stats;  // Squelch read-outs refreshed from the engine\n#endif /* WITH_B200 */\n};\n", "freq_t fields")
@@ -86,7 +86,7 @@ def edit_cmake(t):
     anchor = "if(NOT BCM_VC_FOUND)\n\tpkg_check_modules(FFTW3F REQUIRED fftw3f)"
     if t.count(anchor) != 1:
         raise SystemExit("CMakeLists.txt: anchor not found")
-    add = ('option(WITH_B200 "Demodulate on an NVIDIA B200 through libairband_b200 (github: airband-b200)" OFF)\n'
+    add = ('option(WITH_B200 "Demodulate on an NVIDIA H100 through libairband_b200 (github: airband-b200)" OFF)\n'
            "if(WITH_B200)\n"
            '\tset(B200_ROOT "" CACHE PATH "checkout of the airband-b200 repository (include/, rtlsdr-airband_b200/)")\n'
            "\tadd_definitions(-DWITH_B200 -DABG_WITH_REFERENCE_HEADERS)\n"
