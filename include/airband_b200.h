@@ -240,7 +240,8 @@ ABG_API int abg_debug_k1tc_trace(long long* out);
 ABG_API int abg_debug_k2_stats(unsigned long long* out);
 /* Host-only: plan and coefficient table of the tensor-core K1 (fft_mode 3) for one device, as abg_create builds them
  * (window * twiddle quantised to `digits` signed 8-bit digits, in the shared-memory image the MMA reads).
- * plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups}; tab == NULL queries the plan only. */
+ * plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups} (KBS = k-steps per
+ * shared-memory stage at most, NSTB = stages in the ring); tab == NULL queries the plan only. */
 ABG_API int abg_debug_tc_table(int fft_size, int sfmt, int hop_bytes, float fullscale, int n_channels, const int32_t* bins, int digits,
                                int32_t* plan, signed char* tab, size_t tab_cap, long long* sq, double* cscale);
 

@@ -140,9 +140,10 @@ cudaError_t abg_launch_k1_pruned(const K1Launch& L, const float2* twn, int max_c
 int abg_k1p_tile_frames(int fft_size, int sfmt, int hop_bytes, int max_channels, int* tile_bytes_cap);
 
 // tensor-core variant (k1_tc.cu): the bins' DFT as an integer GEMM on wgmma (8-bit formats, hop_bytes % 32 == 0)
-struct K1TcPlan {
+struct K1TcPlan {  // a ring stage = pps column pairs of a tile (or part of one pair's k-steps); KBS: k-steps per pair and stage at most; NSTB: stages
     int eligible;
     int K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups;
+    int pps;
     size_t table_bytes;
 };
 struct K1TcTables {

@@ -36,6 +36,10 @@ __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// arrive only where `pred` holds, without a branch around it (keeps warp-uniform code between asynchronous MMAs)
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar), "r"((uint32_t)pred) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -116,7 +120,10 @@ __device__ __forceinline__ void mbar_wait_poll(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// arrive on `bar` once every cp.async this thread issued so far has landed (the barrier's count includes this arrival)
+__device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
 // generic-proxy writes (st.shared, cp.async) -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // TMA bulk copy global -> shared, completion counted in bytes on an mbarrier
@@ -135,6 +142,19 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// wait until at most n (warp-uniform; 7 when larger) of the most recent groups are in flight
+__device__ __forceinline__ void wgmma_wait_groups(int n) {
+    switch (n) {
+        case 0: wgmma_wait<0>(); break;
+        case 1: wgmma_wait<1>(); break;
+        case 2: wgmma_wait<2>(); break;
+        case 3: wgmma_wait<3>(); break;
+        case 4: wgmma_wait<4>(); break;
+        case 5: wgmma_wait<5>(); break;
+        case 6: wgmma_wait<6>(); break;
+        default: wgmma_wait<7>(); break;
+    }
+}
 // keeps the compiler from moving accesses of an accumulator register across the asynchronous MMAs that own it
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(uint32_t (&d)[R]) {
@@ -142,10 +162,10 @@ __device__ __forceinline__ void wgmma_fence_regs(uint32_t (&d)[R]) {
     for (int i = 0; i < R; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
 
-// D[64 x N] (+)= A[64 x 32] * B[N x 32]^T for one warpgroup, both operands K-major in shared memory, A unsigned or signed
-// 8-bit (a_signed, warp-uniform), B signed 8-bit, S32 accumulators: thread t of the warpgroup holds d[4j + 2h + e] =
+// D[64 x N] (+)= A[64 x 32] * B[N x 32]^T for one warpgroup, both operands K-major in shared memory, A unsigned (S8 =
+// false) or signed 8-bit, B signed 8-bit, S32 accumulators: thread t of the warpgroup holds d[4j + 2h + e] =
 // D[16 (t / 32) + (t % 32) / 4 + 8h][8j + 2 (t % 4) + e].  acc == 0 overwrites D.
-template <int N>
+template <int N, bool S8>
 struct WgmmaI8;
 // accumulator operand lists, 8 registers at a time, and the matching register strings, 16 at a time
 #define ABG_D8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
@@ -165,30 +185,26 @@ struct WgmmaI8;
 #define ABG_S112 ABG_S96 ", %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111"
 #define ABG_D128 ABG_D112, ABG_D8(112), ABG_D8(120)
 #define ABG_S128 ABG_S112 ", %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
-#define ABG_WGMMA_I8(N, R, P, A, B) \
+#define ABG_WGMMA_I8(N, R, P, A, B, S8, AT) \
     template <> \
-    struct WgmmaI8<N> { \
-        static __device__ __forceinline__ void mma(uint32_t (&d)[R], uint64_t a, uint64_t b, uint32_t acc, uint32_t a_signed) { \
-            if (a_signed) \
-                asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\t" \
-                             "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32.s8.s8 {" ABG_S##R "}, " A ", " B ", p;\n\t}" \
-                             : ABG_D##R \
-                             : "l"(a), "l"(b), "r"(acc)); \
-            else \
-                asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\t" \
-                             "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32.u8.s8 {" ABG_S##R "}, " A ", " B ", p;\n\t}" \
-                             : ABG_D##R \
-                             : "l"(a), "l"(b), "r"(acc)); \
+    struct WgmmaI8<N, S8> { \
+        static __device__ __forceinline__ void mma(uint32_t (&d)[R], uint64_t a, uint64_t b, uint32_t acc) { \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\t" \
+                         "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32." AT ".s8 {" ABG_S##R "}, " A ", " B ", p;\n\t}" \
+                         : ABG_D##R \
+                         : "l"(a), "l"(b), "r"(acc)); \
         } \
     };
-ABG_WGMMA_I8(32, 16, "%18", "%16", "%17")
-ABG_WGMMA_I8(64, 32, "%34", "%32", "%33")
-ABG_WGMMA_I8(96, 48, "%50", "%48", "%49")
-ABG_WGMMA_I8(128, 64, "%66", "%64", "%65")
-ABG_WGMMA_I8(160, 80, "%82", "%80", "%81")
-ABG_WGMMA_I8(192, 96, "%98", "%96", "%97")
-ABG_WGMMA_I8(224, 112, "%114", "%112", "%113")
-ABG_WGMMA_I8(256, 128, "%130", "%128", "%129")
+#define ABG_WGMMA_I8_BOTH(N, R, P, A, B) ABG_WGMMA_I8(N, R, P, A, B, false, "u8") ABG_WGMMA_I8(N, R, P, A, B, true, "s8")
+ABG_WGMMA_I8_BOTH(32, 16, "%18", "%16", "%17")
+ABG_WGMMA_I8_BOTH(64, 32, "%34", "%32", "%33")
+ABG_WGMMA_I8_BOTH(96, 48, "%50", "%48", "%49")
+ABG_WGMMA_I8_BOTH(128, 64, "%66", "%64", "%65")
+ABG_WGMMA_I8_BOTH(160, 80, "%82", "%80", "%81")
+ABG_WGMMA_I8_BOTH(192, 96, "%98", "%96", "%97")
+ABG_WGMMA_I8_BOTH(224, 112, "%114", "%112", "%113")
+ABG_WGMMA_I8_BOTH(256, 128, "%130", "%128", "%129")
+#undef ABG_WGMMA_I8_BOTH
 #undef ABG_WGMMA_I8
 
 }  // namespace tc

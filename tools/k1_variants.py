@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Measurement aid: K1 / K2 durations (CUDA events inside the engine) of one workload for a list of environment-variable
-variants of the tensor-core K1 (stage size, ring size, K-loop rotation, digits), inputs resident.
-    python tools/k1_variants.py cfg2 "ABG_K1_TC_ROTATE=0" "ABG_K1_TC_CAP_KB=227,ABG_K1_TC_STAGE_BYTES=8192" ..."""
+variants of the tensor-core K1 (shared-memory cap, stages in the ring, digits), inputs resident.
+    python tools/k1_variants.py cfg2 "" "ABG_K1_TC_STAGES=4" "ABG_K1_TC_CAP_KB=227" ..."""
 import os
 import sys
 
@@ -20,7 +20,7 @@ def main():
     cfg, desc = bench.make_workload(wname)
     nb = 4
     raws = bench.synth_streams(cfg, nb)
-    knobs = ("ABG_K1_TC_ROTATE", "ABG_K1_TC_CAP_KB", "ABG_K1_TC_STAGE_BYTES", "ABG_K1_TC_STAGES", "ABG_K1_TC_DIGITS", "ABG_K1_TC_NACC", "ABG_K1_TC_SKIP", "FFT_MODE", "ABG_K2_LPW", "ABG_K2_PRIO")
+    knobs = ("ABG_K1_TC_CAP_KB", "ABG_K1_TC_STAGES", "ABG_K1_TC_DIGITS", "FFT_MODE", "ABG_K2_LPW", "ABG_K2_PRIO")
     for v in variants:
         for k in knobs:
             os.environ.pop(k, None)

@@ -29,8 +29,8 @@ buf = np.zeros(256 * 4 * 16 * 4, np.int64)
 assert eng.L.abg_debug_k1tc_trace(buf.ctypes.data_as(C.c_void_p)) == 0
 t = buf.reshape(256, 4, 16, 4)[cta]
 t0 = t[t > 0].min()
-names = {0: ("producer", ["info seen", "empty_a ok", "copies issued", "arrived full_a"]), 1: ("epilogue", ["-", "accumulators ready", "done", "-"]),
-         2: ("loader", ["tile start", "tile B issued", "-", "-"]), 3: ("mma", ["info seen", "full_a ok", "-", "-"])}
+names = {0: ("producer", ["info seen", "-", "-", "tile copies issued"]), 1: ("epilogue", ["-", "accumulators ready", "done", "-"]),
+         2: ("loader", ["tile start", "tile B issued", "-", "-"]), 3: ("mma", ["info seen", "-", "-", "-"])}
 for tile in range(6):
     print(f"tile {tile}")
     for role in range(4):
@@ -38,9 +38,9 @@ for tile in range(6):
         vals = [int(v - t0) if v > 0 else None for v in t[role, tile]]
         print(f"   {nm:9s} " + "  ".join(f"{e}={v}" for e, v in zip(ev, vals) if e != "-"))
 st = buf.reshape(256, 4, 64)[cta]
-print("stage-level stamps of tile 3 (cycles since the loader's first stamp):")
+print("stage-level stamps of tile 3, one stage = one column pair (cycles since the loader's first stamp):")
 base = st[2, 32]
 for k in range(16):
     lo, li, mw, mc = (int(st[2, 32 + 2 * k] - base), int(st[2, 33 + 2 * k] - base), int(st[3, 32 + 2 * k] - base), int(st[3, 33 + 2 * k] - base))
-    print(f"   stage {k:2d}: loader empty_b ok {lo:6d} issued {li:6d} | mma full_b ok {mw:6d} committed {mc:6d}")
+    print(f"   stage {k:2d}: loader empty ok {lo:6d} issued {li:6d} | mma full ok {mw:6d} committed {mc:6d}")
 eng.close()
