@@ -201,6 +201,35 @@ ABG_API int abg_last_run_times(abg_engine* e, float* ms4);
    each of the last n_runs (1..8) runs into ms[5*n_runs]; shows how consecutive runs overlap on the device. */
 ABG_API int abg_debug_timeline(abg_engine* e, int n_runs, float* ms);
 
+/* Band spectrum monitor (not part of the reference surface: the reference opens each SDR exclusively, so there is no
+ * other way to see the band while it runs).  For a device with the monitor on at stride s >= 1, batch b of that device
+ * covers the B = WAVE_BATCH frames whose |X[bin]| fill wavein[AGC_EXTRA + j], j in [0, B); counted from the device's first
+ * frame that is frame f = AGC_EXTRA + b*B + j.  The frames with j % s == 0 are selected, n = ceil(B / s), and
+ *     P[k] = (1/n) * sum over the selected f of |X_f[k]|^2,   k = 0 .. fft_size-1, natural bin order,
+ * where X_f is what fftwf_execute writes at reference src/rtl_airband.cpp:460: the unnormalised forward DFT of the
+ * converted, windowed frame, with the same LUTs, full-scale and Blackman-Harris window as the audio path.  The selection is
+ * relative to the batch, so spectra do not depend on how batches are grouped into runs, and the sums are bitwise
+ * reproducible.  sqrtf(P[k]) is on the scale of the squelch levels: level_to_dBFS(sqrtf(P[k])) (reference
+ * src/util.cpp:169-180) is comparable with abg_squelch_stats.noise_level_dbfs / signal_level_dbfs.  A stride of
+ * ceil(fft_size / hop) selects non-overlapping frames.
+ * Computed on the GPU by one extra kernel per run, after K1 on the K1 stream (it delays the next run's K1, not K2).
+ * With every device off (the default) nothing is launched, allocated or copied.  Resident runs (abg_run_resident) compute
+ * spectra but queue none; batches fed through abg_debug_inject_wavein have no frames and produce no spectrum.
+ *
+ * abg_spectrum_configure: frame_stride 0 = off, >= 1 = on, for batches enqueued by later abg_run / abg_run_resident calls.
+ * ABG_ERANGE for a bad device, ABG_EINVAL for a negative stride.  Waits for the engine's K1 stream. */
+ABG_API int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride);
+/* Pop the oldest unfetched spectrum of a device: power[fft_size] (may be NULL), batch_seq = the device's batch number
+ * among the batches abg_run demodulated since abg_create (0 = the first), n_frames = n.  Returns 1 if one was popped, 0
+ * if none is ready, < 0 on error; waits for the run that computed it.  Lossy by design: a device keeps at most
+ * max_batches_per_run + 2 spectra and a newer one overwrites the oldest (gaps show in batch_seq); the monitor never holds
+ * a result slot or makes abg_run report ABG_EOVERFLOW.  Spectra already queued stay fetchable after the monitor is
+ * switched off or its stride changed. */
+ABG_API int abg_fetch_spectrum(abg_engine* e, int dev, float* power, uint64_t* batch_seq, int32_t* n_frames);
+/* Measurement aid: device time of the spectrum kernel of the most recent run, from CUDA events around it on the K1 stream
+ * (0 if that run computed no spectrum).  Waits for it. */
+ABG_API int abg_debug_spectrum_time(abg_engine* e, float* ms);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

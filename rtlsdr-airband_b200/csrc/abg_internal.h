@@ -160,6 +160,30 @@ void abg_k1tc_build_table(const K1TcPlan& p, int fft_size, int sfmt, const float
 cudaError_t abg_launch_k1_tc(const K1Launch& L, const K1TcPlan& p, const K1TcTables& T, int sm_count, cudaStream_t s);
 int abg_k1tc_trace_dump(long long* out);  // measurement aid (ABG_K1_TC_TRACE): 256*4*16*4 clock64 stamps
 
+// band spectrum monitor (spectrum.cu): see abg_spectrum_configure in include/airband_b200.h
+#define ABG_SPEC_FPC 32  // selected frames per chunk (work item) of one batch
+struct SpecCfg {  // per monitored device; written by abg_spectrum_configure
+    const float* wsc;       // the device's K1 window table (window * 1/full-scale)
+    float* partial;         // [max_batches_per_run][n_chunks][N] chunk sums
+    int32_t* counter;       // [max_batches_per_run] chunks finished per batch; zero between launches
+    float* ring;            // device view of the page-locked result ring [ring_cap][N]
+    int32_t hop_bytes, sfmt, stride, n_sel, n_chunks, ring_cap;
+};
+struct SpecRun {  // per monitored device; uploaded with every run
+    const unsigned char* raw;
+    unsigned long long first_byte;  // first byte of frame j = 0 of the run's first batch
+    int32_t n_batches;              // batches of this run (0 = none)
+    int32_t ring_pos0;              // ring entry of the run's first batch; < 0: resident run, the ring is left alone
+};
+struct SpecArgs {
+    const SpecCfg* cfg;  // [monitored devices]
+    const SpecRun* run;
+    const float2* tw1;
+    const float2* tw2;
+    int wave_batch;
+};
+cudaError_t abg_launch_spectrum(int fft_size, const SpecArgs& a, int n_devices, int max_items, cudaStream_t s);
+
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B
     int lanes_per_warp;       // channels handled by one warp of K2: 1, 2, 4, 8, 16 or 32

@@ -183,6 +183,17 @@ struct Device {
     bool res_primed = false;
     float2* spec = nullptr;  // [nbmax][N] when has_afc
     std::deque<std::pair<int, int>> ready;  // (slot, batch-in-run)
+    uint64_t batch_seq = 0;  // batches of the pushed stream enqueued since abg_create
+    // band spectrum monitor (abg_spectrum_configure); nothing is allocated until it is first switched on
+    int spec_stride = 0, spec_n_sel = 0, spec_chunks = 0;
+    void* spec_work = nullptr;   // device: chunk sums float[nbmax][spec_chunks][N], then the batch counters int32[nbmax]
+    float* spec_ring = nullptr;  // page-locked, mapped: finished spectra [nbmax + 2][N]; kept once allocated
+    int spec_ring_next = 0;      // ring entry of the next spectrum
+    struct SpecEntry {
+        int pos, n_frames;
+        uint64_t seq, run;
+    };
+    std::deque<SpecEntry> spec_ready;  // unfetched spectra, oldest first
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -318,6 +329,14 @@ struct abg_engine {
     cudaEvent_t tl[TL_RUNS][5] = {};
     bool tev_valid = false;
     std::vector<int32_t> h_bins;
+    // band spectrum monitor
+    std::vector<int> spec_devs;              // monitored devices in launch order (grid.y of the spectrum kernel)
+    DevBuf<SpecCfg> spec_cfg;                // [spec_devs.size()]
+    DevBuf<SpecRun> spec_run;                // room for every device
+    std::vector<SpecRun> h_spec_run;
+    cudaEvent_t ev_spec[2] = {nullptr, nullptr};  // after the spectrum kernel of the latest run of each parity (it reads raw[])
+    cudaEvent_t tl_spec[TL_RUNS][2] = {};    // spectrum kernel start / end of the last TL_RUNS runs
+    bool spec_ran[TL_RUNS] = {};
     // mixers (reference src/mixer.cpp)
     int n_mixers = 0;
     DevBuf<int32_t> mix_offsets;
@@ -352,7 +371,13 @@ void engine_free(abg_engine* e) {
             if (d.raw[i]) cudaFree(d.raw[i]);
         if (d.res) cudaFree(d.res);
         if (d.spec) cudaFree(d.spec);
+        if (d.spec_work) cudaFree(d.spec_work);
+        if (d.spec_ring) cudaFreeHost(d.spec_ring);
     }
+    e->spec_cfg.free(); e->spec_run.free();
+    for (auto& row : e->tl_spec)
+        for (auto& ev : row)
+            if (ev) cudaEventDestroy(ev);
     for (auto& g : e->groups) {
         g.wsc.free();
         g.tc_btab.free(); g.tc_sq.free(); g.tc_tab_of_dev.free();
@@ -379,6 +404,7 @@ void engine_free(abg_engine* e) {
     for (int k = 0; k < 2; k++) {
         if (e->ev_k1[k]) cudaEventDestroy(e->ev_k1[k]);
         if (e->ev_k2[k]) cudaEventDestroy(e->ev_k2[k]);
+        if (e->ev_spec[k]) cudaEventDestroy(e->ev_spec[k]);
     }
     if (e->stream_b) cudaStreamDestroy(e->stream_b);
     if (e->stream_c) {
@@ -870,6 +896,44 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     }
     CU(cudaEventRecord(tl[1], sa));
     CU(cudaEventRecord(e->ev_k1[cur], sa));
+    // ---- band spectrum of the monitored devices (stream A: after K1, which K2 does not wait for past ev_k1) ----
+    e->spec_ran[ri % abg_engine::TL_RUNS] = false;
+    if (!skip_k1 && !e->spec_devs.empty()) {
+        int max_items = 0;
+        for (size_t m = 0; m < e->spec_devs.size(); m++) {
+            Device& d = e->dev[e->spec_devs[m]];
+            const int n = nb[e->spec_devs[m]];
+            SpecRun& r = e->h_spec_run[m];
+            const bool primed = resident ? d.res_primed : d.primed;
+            r.raw = resident ? d.res : d.raw[d.cur];
+            // frame j = 0 of the run's first batch: the first AGC_EXTRA frames of a stream only prime the AGC look-back
+            r.first_byte = resident ? (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes
+                                    : (unsigned long long)d.consumed + (primed ? 0ull : (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes);
+            r.n_batches = n;
+            r.ring_pos0 = queue_outputs ? d.spec_ring_next : -1;
+            max_items = std::max(max_items, n * d.spec_chunks);
+            if (!queue_outputs || n <= 0) continue;
+            const int cap = e->nbmax + 2;
+            for (int b = 0; b < n; b++) d.spec_ready.push_back({(d.spec_ring_next + b) % cap, d.spec_n_sel, d.batch_seq + (uint64_t)b, ri});
+            while ((int)d.spec_ready.size() > cap) d.spec_ready.pop_front();  // lossy: the oldest unfetched spectra are overwritten
+            d.spec_ring_next = (d.spec_ring_next + n) % cap;
+        }
+        if (max_items > 0) {
+            const int nl = upload_small(e->spec_run.p, e->h_spec_run.data(), sizeof(SpecRun) * e->spec_devs.size(), sa);
+            if (nl < 0) return fail(ABG_ECUDA, "spectrum parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+            e->launches += (uint64_t)nl;
+            SpecArgs A{};
+            A.cfg = e->spec_cfg.p; A.run = e->spec_run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
+            cudaEvent_t* ts = e->tl_spec[ri % abg_engine::TL_RUNS];
+            CU(cudaEventRecord(ts[0], sa));
+            cudaError_t ers = abg_launch_spectrum(N, A, (int)e->spec_devs.size(), max_items, sa);
+            if (ers != cudaSuccess) return fail(ABG_ECUDA, "spectrum launch failed: %s", cudaGetErrorString(ers));
+            e->launches++;
+            CU(cudaEventRecord(ts[1], sa));
+            CU(cudaEventRecord(e->ev_spec[cur], sa));
+            e->spec_ran[ri % abg_engine::TL_RUNS] = true;
+        }
+    }
     // ---- K2 (stream B, after this run's K1; overlaps the next run's K1) ----
     CU(cudaStreamWaitEvent(sb, e->ev_k1[cur], 0));
     for (size_t i = 0; i < e->dev.size(); i++) {
@@ -943,6 +1007,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             const int frames = nb[i] * B + (d.primed ? 0 : ABG_AGC_EXTRA);
             d.consumed += (size_t)frames * d.hop_bytes;
             d.primed = true;
+            d.batch_seq += (uint64_t)nb[i];
             d.runs_since_compaction++;
         }
     }
@@ -1014,10 +1079,15 @@ int abg_push(abg_engine* e, int dev, const void* iq, size_t nbytes) {
         }
         // the destination buffer was last read by a K1 launched before the previous compaction: with at least one run since
         // then that is run_index-2 or older, so the copy overlaps the K1 that is reading the current buffer right now
+        // (the band spectrum kernel reads the same bytes right after that K1)
         if (d.runs_since_compaction >= 1) {
-            if (e->run_index >= 2) CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 2) & 1], 0));
+            if (e->run_index >= 2) {
+                CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 2) & 1], 0));
+                if (e->ev_spec[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_spec[(e->run_index - 2) & 1], 0));
+            }
         } else if (e->run_index >= 1) {
             CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 1) & 1], 0));
+            if (e->ev_spec[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_spec[(e->run_index - 1) & 1], 0));
         }
         d.runs_since_compaction = 0;
         CU(cudaMemcpyAsync(d.raw[d.cur ^ 1], d.raw[d.cur] + keep_from, rem, cudaMemcpyDeviceToDevice, e->stream_c));
@@ -1172,6 +1242,94 @@ int abg_fft_path(const abg_engine* e, int dev) {
     if (dev < 0 || dev >= (int)e->dev.size()) return ABG_ERANGE;
     const Group& g = e->groups[e->dev[dev].group];
     return g.use_tc ? 3 : (g.pruned ? 2 : 1);
+}
+
+// ---- band spectrum monitor (definition in airband_b200.h) -------------------------------------------------------------
+int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_spectrum_configure: device %d out of range", dev);
+    if (frame_stride < 0) return fail(ABG_EINVAL, "abg_spectrum_configure: frame_stride %d is negative", frame_stride);
+    Device& d = e->dev[dev];
+    if (frame_stride == d.spec_stride) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream));  // an enqueued spectrum kernel may still use the work buffer and the tables
+    const int N = e->N, B = e->B, nbmax = e->nbmax;
+    if (d.spec_work) cudaFree(d.spec_work);
+    d.spec_work = nullptr;
+    d.spec_stride = d.spec_n_sel = d.spec_chunks = 0;
+    if (frame_stride > 0) {
+        if (!e->ev_spec[0]) {
+            for (int k = 0; k < 2; k++) CU(cudaEventCreateWithFlags(&e->ev_spec[k], cudaEventDisableTiming));
+            for (auto& row : e->tl_spec)
+                for (auto& ev : row) CU(cudaEventCreate(&ev));
+        }
+        if (!d.spec_ring) {
+            // unfetched spectra survive later calls (including switching off); the ring lives until abg_destroy
+            if (cudaHostAlloc((void**)&d.spec_ring, sizeof(float) * (size_t)(nbmax + 2) * N, cudaHostAllocMapped) != cudaSuccess) {
+                d.spec_ring = nullptr;
+                return fail(ABG_ENOMEM, "Out of page-locked host memory for the spectrum ring");
+            }
+        }
+        const int n_sel = (B + frame_stride - 1) / frame_stride;
+        const int chunks = (n_sel + ABG_SPEC_FPC - 1) / ABG_SPEC_FPC;
+        const size_t sums = sizeof(float) * (size_t)nbmax * chunks * N;
+        if (cudaMalloc(&d.spec_work, sums + sizeof(int32_t) * nbmax) != cudaSuccess) {
+            d.spec_work = nullptr;
+            return fail(ABG_ENOMEM, "Out of device memory for the spectrum of device %d", dev);
+        }
+        CU(cudaMemset(static_cast<char*>(d.spec_work) + sums, 0, sizeof(int32_t) * nbmax));
+        d.spec_stride = frame_stride;
+        d.spec_n_sel = n_sel;
+        d.spec_chunks = chunks;
+    }
+    // rebuild the launch's device list and its static table
+    e->spec_devs.clear();
+    std::vector<SpecCfg> cfgs;
+    for (int i = 0; i < (int)e->dev.size(); i++) {
+        const Device& x = e->dev[i];
+        if (x.spec_stride <= 0) continue;
+        SpecCfg c{};
+        c.wsc = e->groups[x.group].wsc.p;
+        c.partial = static_cast<float*>(x.spec_work);
+        c.counter = reinterpret_cast<int32_t*>(static_cast<char*>(x.spec_work) + sizeof(float) * (size_t)nbmax * x.spec_chunks * N);
+        CU(cudaHostGetDevicePointer((void**)&c.ring, x.spec_ring, 0));
+        c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = x.spec_stride; c.n_sel = x.spec_n_sel; c.n_chunks = x.spec_chunks;
+        c.ring_cap = nbmax + 2;
+        e->spec_devs.push_back(i);
+        cfgs.push_back(c);
+    }
+    e->spec_cfg.free();
+    e->h_spec_run.assign(e->spec_devs.size(), SpecRun{});
+    if (cfgs.empty()) return ABG_OK;
+    if (e->spec_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the spectrum tables");
+    CU(cudaMemcpy(e->spec_cfg.p, cfgs.data(), sizeof(SpecCfg) * cfgs.size(), cudaMemcpyHostToDevice));
+    // upload_small writes whole 16-byte words: room for every device plus the rounding
+    if (!e->spec_run.p && e->spec_run.alloc(e->dev.size() + 1)) return fail(ABG_ENOMEM, "Out of device memory for the spectrum tables");
+    return ABG_OK;
+}
+
+int abg_fetch_spectrum(abg_engine* e, int dev, float* power, uint64_t* batch_seq, int32_t* n_frames) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_spectrum: device %d out of range", dev);
+    Device& d = e->dev[dev];
+    if (d.spec_ready.empty()) return 0;
+    const Device::SpecEntry r = d.spec_ready.front();
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaEventSynchronize(e->tl_spec[r.run % abg_engine::TL_RUNS][1]));  // (a later record of it is a later run: also fine)
+    if (power) memcpy(power, d.spec_ring + (size_t)r.pos * e->N, sizeof(float) * e->N);
+    if (batch_seq) *batch_seq = r.seq;
+    if (n_frames) *n_frames = r.n_frames;
+    d.spec_ready.pop_front();
+    return 1;
+}
+
+int abg_debug_spectrum_time(abg_engine* e, float* ms) {
+    if (!ms) return fail(ABG_EINVAL, "abg_debug_spectrum_time: null argument");
+    *ms = 0.0f;
+    if (e->run_index == 0 || !e->spec_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    cudaEvent_t* ts = e->tl_spec[(e->run_index - 1) % abg_engine::TL_RUNS];
+    CU(cudaEventSynchronize(ts[1]));
+    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
+    return ABG_OK;
 }
 
 // ---- scan mode -------------------------------------------------------------------------------------------------------

@@ -12,7 +12,7 @@
 //     the tile's raw bytes ((TF-1)*hop + N samples) ONCE in shared memory with a single TMA bulk copy
 //     (cp.async.bulk ... mbarrier::complete_tx) and every frame converts from there: HBM sees each input byte
 //     about once per tile (+ the N-hop overlap between neighbouring tiles, which hits L2).
-//   * an N-point FFT is 2 (3 for N=8192) register passes: each thread holds one radix-R1 column in registers
+//   * an N-point FFT (fft_frame() in k1_fft.cuh, shared with the band-spectrum kernel) is 2 (3 for N=8192) register passes: each thread holds one radix-R1 column in registers
 //     (R1 up to 64 complex values), runs a fully unrolled decimation-in-time FFT on it whose twiddles are
 //     compile-time immediates, applies the inter-pass twiddle, and exchanges through a padded shared-memory
 //     buffer; the last pass leaves bin k1 + R1*k2 in register k2 of thread k1.
@@ -32,36 +32,10 @@
 #include "../../include/airband_b200.h"
 #include "abg_internal.h"
 #include "k1_common.cuh"
+#include "k1_fft.cuh"
 
 namespace {
 using namespace k1;
-
-// ---------------------------------------------------------------------------------------------------------------
-// per-size plan
-// ---------------------------------------------------------------------------------------------------------------
-template <int LOGN>
-struct Plan;
-template <>
-struct Plan<8> { static constexpr int R1 = 16, R2 = 16, R3 = 0, T = 16, BLOCK = 128; };
-template <>
-struct Plan<9> { static constexpr int R1 = 32, R2 = 16, R3 = 0, T = 16, BLOCK = 128; };
-template <>
-struct Plan<10> { static constexpr int R1 = 32, R2 = 32, R3 = 0, T = 32, BLOCK = 128; };
-template <>
-struct Plan<11> { static constexpr int R1 = 64, R2 = 32, R3 = 0, T = 32, BLOCK = 128; };
-template <>
-struct Plan<12> { static constexpr int R1 = 64, R2 = 64, R3 = 0, T = 64, BLOCK = 128; };
-template <>
-struct Plan<13> { static constexpr int R1 = 32, R2 = 16, R3 = 16, T = 256, BLOCK = 256; };
-
-template <int T>
-__device__ __forceinline__ void frame_sync(int slot) {
-    if constexpr (T <= 32) {
-        __syncwarp();
-    } else {
-        asm volatile("bar.sync %0, %1;" ::"r"(slot + 1), "r"(T) : "memory");
-    }
-}
 
 struct K1Args {
     const K1Dev* devs;
@@ -106,15 +80,11 @@ __device__ __forceinline__ void emit_bins(const float2 (&v)[R], unsigned long lo
 template <int LOGN, int SFMT>
 __global__ void __launch_bounds__(Plan<LOGN>::BLOCK) k1_fft_kernel(const K1Args a) {
     using P = Plan<LOGN>;
-    constexpr int N = 1 << LOGN;
-    constexpr int R1 = P::R1, R2 = P::R2, R3 = P::R3, T = P::T, BLOCK = P::BLOCK;
-    constexpr bool THREE = R3 != 0;
-    constexpr int RL = THREE ? R3 : R2;       // last-pass radix
-    constexpr int M1 = N / R1;                // pass-1 butterflies per frame (= sub-transform length after pass 1)
-    constexpr int S = BLOCK / T;              // frames in flight per CTA
-    constexpr int PADSH = ilog2(RL);          // exchange padding: one float2 every RL
-    constexpr int EXN = N + (N >> PADSH);     // padded exchange elements per frame
-    constexpr int NQL = N / RL;               // last-pass butterflies per frame
+    using F = FftShape<LOGN>;
+    constexpr int N = F::N;
+    constexpr int R1 = P::R1, R2 = P::R2, T = P::T, BLOCK = P::BLOCK;
+    constexpr bool THREE = F::THREE;
+    constexpr int RL = F::RL, S = F::S, EXN = F::EXN, NQL = F::NQL;
     constexpr int BPC = bytes_per_cplx<SFMT>();
     static_assert(S >= 1, "block too small");
 
@@ -178,15 +148,6 @@ __global__ void __launch_bounds__(Plan<LOGN>::BLOCK) k1_fft_kernel(const K1Args 
 
     const int slot = tid / T, lt = tid % T;
     float2* ex = ex_all + (size_t)slot * EXN;
-    const float* __restrict__ wsc = a.wsc;
-    const float2* __restrict__ tw1 = a.tw1;
-
-    auto bin_of = [](int q, int r) -> int {
-        if constexpr (!THREE)
-            return q + R1 * r;
-        else
-            return (q / R2) + R1 * ((q % R2) + R2 * r);
-    };
 
     const int iters = (nf + S - 1) / S;
     for (int it = 0; it < iters; ++it) {
@@ -197,90 +158,9 @@ __global__ void __launch_bounds__(Plan<LOGN>::BLOCK) k1_fft_kernel(const K1Args 
         float2* spec_row = nullptr;
         if (active && dv.spec != nullptr && pos >= dv.spec_first_pos && ((pos - dv.spec_first_pos) % dv.wave_batch) == 0)
             spec_row = dv.spec + (size_t)((pos - dv.spec_first_pos) / dv.wave_batch) * N;
-
-        // ---------------- pass 1: radix-R1 columns, window fused into the load -----------------------------
-        if (active) {
-#pragma unroll 1
-            for (int n2 = lt; n2 < M1; n2 += T) {
-                float2 v[R1];
-#pragma unroll
-                for (int n1 = 0; n1 < R1; ++n1) {
-                    const int n = n2 + M1 * n1;
-                    const float2 x = load_sample<SFMT>(tile, fo + n * BPC);
-                    const float w = __ldg(wsc + n);
-                    v[n1] = make_float2(x.x * w, x.y * w);
-                }
-                reg_fft<R1>(v);
-                ex[n2 + (n2 >> PADSH)] = v[0];
-#pragma unroll
-                for (int k1 = 1; k1 < R1; ++k1) {
-                    const float2 t = __ldg(tw1 + k1 * M1 + n2);
-                    const float2 y = v[brev<R1>(k1)];
-                    const int e = k1 * M1 + n2;
-                    ex[e + (e >> PADSH)] = make_float2(fmaf(-y.y, t.y, y.x * t.x), fmaf(y.y, t.x, y.x * t.y));
-                }
-            }
-        }
-        frame_sync<T>(slot);
-
-        if constexpr (!THREE) {
-            // ------------- pass 2 (last): rows of length R2 = M1; bin k1 + R1*k2 ends up in register k2 -------
-            if (active) {
-#pragma unroll 1
-                for (int q = lt; q < NQL; q += T) {
-                    float2 v[R2];
-#pragma unroll
-                    for (int j = 0; j < R2; ++j) {
-                        const int e = q * M1 + j;
-                        v[j] = ex[e + (e >> PADSH)];
-                    }
-                    reg_fft<R2>(v);
-                    emit_bins<R2>(v, want[q], q, dv, a, pos, spec_row, bin_of);
-                }
-            }
-        } else {
-            // ------------- pass 2 of 3: radix R2 inside each length-M1 block, twiddle W_M1^(n3*k2a) ------------
-            constexpr int M2 = R3;
-            const float2* __restrict__ tw2 = a.tw2;
-            if (active) {
-#pragma unroll 1
-                for (int q = lt; q < N / R2; q += T) {
-                    const int k1 = q / M2, n3 = q % M2;
-                    const int base = k1 * M1 + n3;
-                    float2 v[R2];
-#pragma unroll
-                    for (int j = 0; j < R2; ++j) {
-                        const int e = base + M2 * j;
-                        v[j] = ex[e + (e >> PADSH)];
-                    }
-                    reg_fft<R2>(v);
-                    ex[base + (base >> PADSH)] = v[0];
-#pragma unroll
-                    for (int k = 1; k < R2; ++k) {
-                        const float2 t = __ldg(tw2 + k * M2 + n3);
-                        const float2 y = v[brev<R2>(k)];
-                        const int e = base + M2 * k;
-                        ex[e + (e >> PADSH)] = make_float2(fmaf(-y.y, t.y, y.x * t.x), fmaf(y.y, t.x, y.x * t.y));
-                    }
-                }
-            }
-            frame_sync<T>(slot);
-            // ------------- pass 3 (last) -----------------------------------------------------------------------
-            if (active) {
-#pragma unroll 1
-                for (int q = lt; q < NQL; q += T) {
-                    float2 v[R3 == 0 ? 1 : R3];
-#pragma unroll
-                    for (int j = 0; j < R3; ++j) {
-                        const int e = q * R3 + j;
-                        v[j] = ex[e + (e >> PADSH)];
-                    }
-                    reg_fft<(R3 == 0 ? 1 : R3)>(v);
-                    emit_bins<(R3 == 0 ? 1 : R3)>(v, want[q], q, dv, a, pos, spec_row, bin_of);
-                }
-            }
-        }
-        frame_sync<T>(slot);  // exchange buffer is reused by this slot's next frame
+        fft_frame<LOGN, SFMT>(tile + fo, active, slot, lt, ex, a.wsc, a.tw1, a.tw2, [&](const float2(&v)[RL], int q) {
+            emit_bins<RL>(v, want[q], q, dv, a, pos, spec_row, F::bin_of);
+        });
     }
 }
 

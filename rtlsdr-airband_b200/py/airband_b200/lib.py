@@ -23,7 +23,7 @@ SYMBOLS = [
     "abg_batches_available", "abg_run", "abg_sync", "abg_join", "abg_batches_ready", "abg_fetch_batch", "abg_fetch_batches", "abg_get_stats", "abg_set_bin",
     "abg_resident_load", "abg_run_resident", "abg_set_stream", "abg_launch_count", "abg_mixers_configure",
     "abg_fetch_mixer_batch", "abg_mixer_device_buffers", "abg_debug_frame", "abg_last_run_times", "abg_debug_timeline", "abg_scan_configure", "abg_scan_select", "abg_host_register", "abg_host_unregister", "abg_ingest_sync", "abg_fft_path", "abg_debug_tc_table", "abg_debug_inject_wavein", "abg_debug_k1tc_trace", "abg_debug_k2_stats",
-    "abg_debug_run_outputs",
+    "abg_debug_run_outputs", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
 ]
 
 
@@ -96,6 +96,10 @@ def load():
     L.abg_debug_inject_wavein.restype, L.abg_debug_inject_wavein.argtypes = i, [vp, i, i, vp]
     L.abg_debug_k1tc_trace.restype, L.abg_debug_k1tc_trace.argtypes = i, [vp]
     L.abg_debug_k2_stats.restype, L.abg_debug_k2_stats.argtypes = i, [vp]
+    L.abg_spectrum_configure.restype, L.abg_spectrum_configure.argtypes = i, [vp, i, i]
+    L.abg_fetch_spectrum.restype = i
+    L.abg_fetch_spectrum.argtypes = [vp, i, vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
+    L.abg_debug_spectrum_time.restype, L.abg_debug_spectrum_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -251,6 +255,27 @@ class Engine:
     def launch_count(self) -> int:
         return int(self.L.abg_launch_count(self.h))
 
+    # ---- band spectrum monitor -----------------------------------------------------------------------------------
+    def spectrum_configure(self, dev: int, stride: int) -> None:
+        """Batch-averaged power spectrum of a device every `stride`-th frame of each batch (0 = off, the default); applies
+        to batches enqueued by later runs.  `default_stride(cfg, dev)` selects non-overlapping frames."""
+        self._chk(self.L.abg_spectrum_configure(self.h, dev, stride))
+
+    def fetch_spectrum(self, dev: int) -> Optional[Tuple[np.ndarray, int, int]]:
+        """Oldest unfetched spectrum of a device: (power[fft_size] float32, batch_seq, n_frames), or None.  Lossy: at most
+        max_batches_per_run + 2 are kept per device."""
+        p = np.empty(self.cfg.fft_size, np.float32)
+        seq, nf = C.c_uint64(0), C.c_int32(0)
+        if not self._chk(self.L.abg_fetch_spectrum(self.h, dev, _ptr(p), C.byref(seq), C.byref(nf))):
+            return None
+        return p, int(seq.value), int(nf.value)
+
+    def spectrum_time(self) -> float:
+        """ms of the spectrum kernel in the most recent run (CUDA events on the K1 stream); 0 if it computed none."""
+        ms = C.c_float(0.0)
+        self._chk(self.L.abg_debug_spectrum_time(self.h, C.byref(ms)))
+        return float(ms.value)
+
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
         """mixers[m] = [(dev, chan, ampfactor, balance), ...]"""
@@ -290,6 +315,22 @@ class Engine:
         raw_frame = np.ascontiguousarray(raw_frame)
         self._chk(self.L.abg_debug_frame(self.h, dev, _ptr(raw_frame), _ptr(out)))
         return out.view(np.complex64)
+
+
+def default_stride(cfg: Config, dev: int) -> int:
+    """ceil(fft_size / hop): the spectrum stride that selects non-overlapping frames of a device."""
+    return -(-cfg.fft_size // cfg.hop(dev))
+
+
+def spectrum_dbfs(power: np.ndarray, fft_size: int) -> np.ndarray:
+    """level_to_dBFS(sqrtf(P)) per bin (reference src/util.cpp:169-180), the scale of abg_squelch_stats' *_dbfs fields:
+    min(0, 20*log10f(level / fft_size) + 7.54 + 10*log10f(fft_size / 2) - 2.38), in float32.  A zero bin gives -inf."""
+    f32 = np.float32
+    level = np.sqrt(np.asarray(power, np.float32))
+    offset = f32(f32(7.54) + f32(10.0) * np.log10(f32(fft_size // 2))) - f32(2.38)
+    with np.errstate(divide="ignore"):
+        db = f32(20.0) * np.log10(level / f32(fft_size)) + offset
+    return np.minimum(f32(0.0), db.astype(np.float32))
 
 
 TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "acc_regs", "smem_bytes", "halo", "consumer_warpgroups")
