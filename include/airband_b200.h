@@ -230,6 +230,50 @@ ABG_API int abg_fetch_spectrum(abg_engine* e, int dev, float* power, uint64_t* b
  * (0 if that run computed no spectrum).  Waits for it. */
 ABG_API int abg_debug_spectrum_time(abg_engine* e, float* ms);
 
+/* Carrier frequency meter (not part of the reference surface: it shows how far each transmitter sits from its configured
+ * frequency while the engine holds the SDRs, to well below one FFT bin).  For a device with the meter on, batch b covers
+ * the same B = WAVE_BATCH frames as the band spectrum, f_j = AGC_EXTRA + b*B + j, j in [0, B).  With X_f the value of the
+ * channel's bin in frame f (channel_t.iq_in, reference src/rtl_airband.cpp:483-489; the bin the batch used, so AFC moves
+ * it between batches), for every channel c
+ *     R[c] = sum_{j=0}^{B-2} X_{f_{j+1}} * conj(X_{f_j})    (complex, float32)
+ *     E[c] = sum_{j=0}^{B-1} |X_{f_j}|^2                     (float32)
+ * Only pairs inside the batch count, so the results do not depend on how batches are grouped into runs, and the sums are
+ * bitwise reproducible (fixed reduction order).
+ * Consecutive frames start hop = abg_hop() samples apart, so a tone at baseband frequency f gives X_{f+1} = X_f *
+ * exp(2*pi*i * f * hop / sample_rate) for any bin of its main lobe: arg(R) / (2*pi) is f * hop / sample_rate modulo 1.
+ * An AM envelope leaves the phase alone, and a symmetric FM tone of peak deviation D shrinks |R| by
+ * J0(2*pi*D*hop/sample_rate) and keeps its direction while that is positive (D below about 3 kHz at 8000 frames/s), as
+ * long as the window weighs the upper and lower sidebands alike.  Once the carrier is off its bin's centre they are
+ * weighed unequally and the reading is biased towards the stronger one: with the 7-term Blackman-Harris window, a 60 % AM
+ * tone at 1 kHz 3.5 kHz from the centre reads about 4 Hz off in a 10 kHz bin and 0.3 Hz off in a 39 kHz bin, NFM with
+ * D = 2.5 kHz about 180 Hz and 15 Hz off; a steady carrier reads exactly.  The carrier's error relative
+ * to the configured frequency, unambiguous within +-sample_rate / (2*hop) (about +-WAVE_RATE/2), is
+ *     offset_hz = wrap(arg(R) / (2*pi) - channel_offset_hz * hop / sample_rate) * sample_rate / hop,  wrap to [-0.5, 0.5)
+ * with channel_offset_hz = freq - centerfreq of the configured channel (or of the scan entry the batch used); use hop, not
+ * WAVE_RATE, when sample_rate / WAVE_RATE is not an integer (as calc_dm_dphi does, reference src/config.cpp:679-712).
+ * |R| / E lies in [0, 1] (Cauchy-Schwarz): about 1 for a carrier with a steady envelope, 0.955 for a 60 % AM tone at
+ * 1 kHz.  It is NOT a noise gate: consecutive frames overlap, so white noise alone gives |R| / E ~ rho_w(hop) =
+ * sum w[n] w[n+hop] / sum w[n]^2 of the Blackman-Harris window, with its phase at the bin centre: 0 when fft_size <= hop,
+ * 0.59 at fft_size 2048 / hop 320, 0.92 at 4096 / 256, 0.98 at 8192 / 256.  Read the offset on batches whose
+ * axcindicate shows a signal: the squelch is the gate.
+ * Computed on the GPU by one extra kernel per run on the K1 stream, after K1 (and after the band spectrum when that is
+ * on); K2 does not wait for it.  With every device off (the default) nothing is launched, allocated or copied.
+ * Resident runs (abg_run_resident) compute the sums but queue none; batches fed through abg_debug_inject_wavein have no
+ * frames and produce none.
+ *
+ * abg_carrier_configure: on = 1 / 0 switches the meter on / off for batches enqueued by later abg_run / abg_run_resident
+ * calls.  ABG_ERANGE for a bad device, ABG_EINVAL for any other value of on.  Waits for the engine's K1 stream. */
+ABG_API int abg_carrier_configure(abg_engine* e, int dev, int on);
+/* Pop the oldest unfetched meter reading of a device: lag1[n_channels][2] = R (re, im), energy[n_channels] = E (either may
+ * be NULL), batch_seq numbered as for abg_fetch_spectrum.  Returns 1 if one was popped, 0 if none is ready, < 0 on error;
+ * waits for the run that computed it.  The queue is lossy exactly like the spectrum's: max_batches_per_run + 2 readings
+ * per device, the oldest overwritten first; the meter never holds a result slot or causes ABG_EOVERFLOW, and readings
+ * already queued stay fetchable after the meter is switched off. */
+ABG_API int abg_fetch_carrier(abg_engine* e, int dev, float* lag1, float* energy, uint64_t* batch_seq);
+/* Measurement aid: device time of the meter kernel of the most recent run, from CUDA events around it on the K1 stream
+ * (0 if that run metered nothing).  Waits for it. */
+ABG_API int abg_debug_carrier_time(abg_engine* e, float* ms);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

@@ -184,6 +184,24 @@ struct SpecArgs {
 };
 cudaError_t abg_launch_spectrum(int fft_size, const SpecArgs& a, int n_devices, int max_items, cudaStream_t s);
 
+// carrier frequency meter (carrier.cu): see abg_carrier_configure in include/airband_b200.h
+struct CarCfg {  // per metered device; written by abg_carrier_configure
+    float* ring;         // device view of the page-locked result ring [ring_cap][3 * n_channels]: lag1 re/im pairs, then energies
+    int32_t g0, n_channels, ring_cap;
+};
+struct CarRun {  // per metered device; uploaded with every run
+    int32_t n_batches;  // batches of this run (0 = none)
+    int32_t ring_pos0;  // ring entry of the run's first batch; < 0: resident run, the ring is left alone
+};
+struct CarArgs {
+    const CarCfg* cfg;  // [metered devices]
+    const CarRun* run;
+    const float2* iqin;  // [P][Gp] the run's K1 output
+    int Gp, wave_batch;
+};
+cudaError_t abg_launch_carrier(const CarArgs& a, int n_devices, int max_items, cudaStream_t s);
+int abg_carrier_items(int n_channels);  // work items per batch of a device
+
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B
     int lanes_per_warp;       // channels handled by one warp of K2: 1, 2, 4, 8, 16 or 32

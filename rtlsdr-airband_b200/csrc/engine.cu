@@ -167,6 +167,46 @@ struct DevBuf {
     }
 };
 
+// Result queue of one device's batch monitor (band spectrum, carrier meter).  The monitor's kernel writes the result of
+// every batch straight into a page-locked, mapped ring of `cap` = max_batches_per_run + 2 entries; the host keeps the
+// unfetched entries, oldest first.  Lossy by design: queueing a run drops the oldest unfetched entries beyond the ring's
+// size (gaps show in their batch_seq), so a monitor never holds a result slot or causes ABG_EOVERFLOW.
+struct MonitorQueue {
+    struct Entry {
+        int pos;           // ring entry
+        int32_t n_frames;  // monitor-specific count (spectrum: frames averaged)
+        uint64_t seq, run;
+    };
+    unsigned char* ring = nullptr;  // [cap][entry_bytes]; allocated when the monitor is first switched on, kept until abg_destroy
+    size_t entry_bytes = 0;
+    int cap = 0, next = 0;
+    std::deque<Entry> ready;
+
+    // false: out of page-locked memory.  Entries already queued survive (switching a monitor off and on keeps them).
+    bool alloc(int cap_, size_t entry_bytes_) {
+        if (ring) return true;
+        if (cudaHostAlloc((void**)&ring, (size_t)cap_ * entry_bytes_, cudaHostAllocMapped) != cudaSuccess) {
+            ring = nullptr;
+            return false;
+        }
+        cap = cap_;
+        entry_bytes = entry_bytes_;
+        return true;
+    }
+    void release() {
+        if (ring) cudaFreeHost(ring);
+        ring = nullptr;
+    }
+    // Queue the n batches of run `run` whose first is batch number seq0; returns the ring entry of the first.
+    int queue(int n, uint64_t seq0, uint64_t run, int32_t n_frames) {
+        const int pos0 = next;
+        for (int b = 0; b < n; b++) ready.push_back({(next + b) % cap, n_frames, seq0 + (uint64_t)b, run});
+        while ((int)ready.size() > cap) ready.pop_front();
+        next = (next + n) % cap;
+        return pos0;
+    }
+};
+
 struct Device {
     int sfmt = 0, bpc = 0, sample_rate = 0, hop = 0, hop_bytes = 0;
     float fullscale = 0;
@@ -187,13 +227,10 @@ struct Device {
     // band spectrum monitor (abg_spectrum_configure); nothing is allocated until it is first switched on
     int spec_stride = 0, spec_n_sel = 0, spec_chunks = 0;
     void* spec_work = nullptr;   // device: chunk sums float[nbmax][spec_chunks][N], then the batch counters int32[nbmax]
-    float* spec_ring = nullptr;  // page-locked, mapped: finished spectra [nbmax + 2][N]; kept once allocated
-    int spec_ring_next = 0;      // ring entry of the next spectrum
-    struct SpecEntry {
-        int pos, n_frames;
-        uint64_t seq, run;
-    };
-    std::deque<SpecEntry> spec_ready;  // unfetched spectra, oldest first
+    MonitorQueue spec_q;         // finished spectra float[N] per entry
+    // carrier frequency meter (abg_carrier_configure); nothing is allocated until it is first switched on
+    bool car_on = false;
+    MonitorQueue car_q;          // lag1 float[C][2], then energy float[C] per entry
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -337,6 +374,13 @@ struct abg_engine {
     cudaEvent_t ev_spec[2] = {nullptr, nullptr};  // after the spectrum kernel of the latest run of each parity (it reads raw[])
     cudaEvent_t tl_spec[TL_RUNS][2] = {};    // spectrum kernel start / end of the last TL_RUNS runs
     bool spec_ran[TL_RUNS] = {};
+    // carrier frequency meter
+    std::vector<int> car_devs;               // metered devices in launch order (grid.y of the meter kernel)
+    DevBuf<CarCfg> car_cfg;                  // [car_devs.size()]
+    DevBuf<CarRun> car_run;                  // room for every device
+    std::vector<CarRun> h_car_run;
+    cudaEvent_t tl_car[TL_RUNS][2] = {};     // meter kernel start / end of the last TL_RUNS runs
+    bool car_ran[TL_RUNS] = {};
     // mixers (reference src/mixer.cpp)
     int n_mixers = 0;
     DevBuf<int32_t> mix_offsets;
@@ -372,10 +416,15 @@ void engine_free(abg_engine* e) {
         if (d.res) cudaFree(d.res);
         if (d.spec) cudaFree(d.spec);
         if (d.spec_work) cudaFree(d.spec_work);
-        if (d.spec_ring) cudaFreeHost(d.spec_ring);
+        d.spec_q.release();
+        d.car_q.release();
     }
     e->spec_cfg.free(); e->spec_run.free();
+    e->car_cfg.free(); e->car_run.free();
     for (auto& row : e->tl_spec)
+        for (auto& ev : row)
+            if (ev) cudaEventDestroy(ev);
+    for (auto& row : e->tl_car)
         for (auto& ev : row)
             if (ev) cudaEventDestroy(ev);
     for (auto& g : e->groups) {
@@ -910,13 +959,8 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             r.first_byte = resident ? (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes
                                     : (unsigned long long)d.consumed + (primed ? 0ull : (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes);
             r.n_batches = n;
-            r.ring_pos0 = queue_outputs ? d.spec_ring_next : -1;
+            r.ring_pos0 = queue_outputs && n > 0 ? d.spec_q.queue(n, d.batch_seq, ri, d.spec_n_sel) : -1;
             max_items = std::max(max_items, n * d.spec_chunks);
-            if (!queue_outputs || n <= 0) continue;
-            const int cap = e->nbmax + 2;
-            for (int b = 0; b < n; b++) d.spec_ready.push_back({(d.spec_ring_next + b) % cap, d.spec_n_sel, d.batch_seq + (uint64_t)b, ri});
-            while ((int)d.spec_ready.size() > cap) d.spec_ready.pop_front();  // lossy: the oldest unfetched spectra are overwritten
-            d.spec_ring_next = (d.spec_ring_next + n) % cap;
         }
         if (max_items > 0) {
             const int nl = upload_small(e->spec_run.p, e->h_spec_run.data(), sizeof(SpecRun) * e->spec_devs.size(), sa);
@@ -932,6 +976,34 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             CU(cudaEventRecord(ts[1], sa));
             CU(cudaEventRecord(e->ev_spec[cur], sa));
             e->spec_ran[ri % abg_engine::TL_RUNS] = true;
+        }
+    }
+    // ---- carrier meter of the metered devices (stream A: after K1 and the spectrum; reads iqin[cur], which the next
+    // K1 to write it, two runs later, queues behind on this stream) ----
+    e->car_ran[ri % abg_engine::TL_RUNS] = false;
+    if (!skip_k1 && !e->car_devs.empty()) {
+        int max_items = 0;
+        for (size_t m = 0; m < e->car_devs.size(); m++) {
+            Device& d = e->dev[e->car_devs[m]];
+            const int n = nb[e->car_devs[m]];
+            CarRun& r = e->h_car_run[m];
+            r.n_batches = n;
+            r.ring_pos0 = queue_outputs && n > 0 ? d.car_q.queue(n, d.batch_seq, ri, 0) : -1;
+            max_items = std::max(max_items, n * abg_carrier_items(d.C));
+        }
+        if (max_items > 0) {
+            const int nl = upload_small(e->car_run.p, e->h_car_run.data(), sizeof(CarRun) * e->car_devs.size(), sa);
+            if (nl < 0) return fail(ABG_ECUDA, "carrier meter parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+            e->launches += (uint64_t)nl;
+            CarArgs A{};
+            A.cfg = e->car_cfg.p; A.run = e->car_run.p; A.iqin = e->iqin[cur].p; A.Gp = e->Gp; A.wave_batch = B;
+            cudaEvent_t* ts = e->tl_car[ri % abg_engine::TL_RUNS];
+            CU(cudaEventRecord(ts[0], sa));
+            cudaError_t erc = abg_launch_carrier(A, (int)e->car_devs.size(), max_items, sa);
+            if (erc != cudaSuccess) return fail(ABG_ECUDA, "carrier meter launch failed: %s", cudaGetErrorString(erc));
+            e->launches++;
+            CU(cudaEventRecord(ts[1], sa));
+            e->car_ran[ri % abg_engine::TL_RUNS] = true;
         }
     }
     // ---- K2 (stream B, after this run's K1; overlaps the next run's K1) ----
@@ -1262,13 +1334,7 @@ int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
             for (auto& row : e->tl_spec)
                 for (auto& ev : row) CU(cudaEventCreate(&ev));
         }
-        if (!d.spec_ring) {
-            // unfetched spectra survive later calls (including switching off); the ring lives until abg_destroy
-            if (cudaHostAlloc((void**)&d.spec_ring, sizeof(float) * (size_t)(nbmax + 2) * N, cudaHostAllocMapped) != cudaSuccess) {
-                d.spec_ring = nullptr;
-                return fail(ABG_ENOMEM, "Out of page-locked host memory for the spectrum ring");
-            }
-        }
+        if (!d.spec_q.alloc(nbmax + 2, sizeof(float) * N)) return fail(ABG_ENOMEM, "Out of page-locked host memory for the spectrum ring");
         const int n_sel = (B + frame_stride - 1) / frame_stride;
         const int chunks = (n_sel + ABG_SPEC_FPC - 1) / ABG_SPEC_FPC;
         const size_t sums = sizeof(float) * (size_t)nbmax * chunks * N;
@@ -1291,7 +1357,7 @@ int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
         c.wsc = e->groups[x.group].wsc.p;
         c.partial = static_cast<float*>(x.spec_work);
         c.counter = reinterpret_cast<int32_t*>(static_cast<char*>(x.spec_work) + sizeof(float) * (size_t)nbmax * x.spec_chunks * N);
-        CU(cudaHostGetDevicePointer((void**)&c.ring, x.spec_ring, 0));
+        CU(cudaHostGetDevicePointer((void**)&c.ring, x.spec_q.ring, 0));
         c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = x.spec_stride; c.n_sel = x.spec_n_sel; c.n_chunks = x.spec_chunks;
         c.ring_cap = nbmax + 2;
         e->spec_devs.push_back(i);
@@ -1307,17 +1373,28 @@ int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
     return ABG_OK;
 }
 
+// Pop the oldest entry of a monitor queue once the monitor kernel of its run (end events `ends`) has finished: returns 1
+// and the entry's ring bytes in *data, 0 if the queue is empty, < 0 on error.
+static int monitor_pop(abg_engine* e, MonitorQueue& q, cudaEvent_t (&ends)[abg_engine::TL_RUNS][2], const unsigned char** data,
+                       MonitorQueue::Entry* got) {
+    if (q.ready.empty()) return 0;
+    *got = q.ready.front();
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaEventSynchronize(ends[got->run % abg_engine::TL_RUNS][1]));  // (a later record of it is a later run: also fine)
+    *data = q.ring + (size_t)got->pos * q.entry_bytes;
+    q.ready.pop_front();  // the bytes stay put until a later run is enqueued
+    return 1;
+}
+
 int abg_fetch_spectrum(abg_engine* e, int dev, float* power, uint64_t* batch_seq, int32_t* n_frames) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_spectrum: device %d out of range", dev);
-    Device& d = e->dev[dev];
-    if (d.spec_ready.empty()) return 0;
-    const Device::SpecEntry r = d.spec_ready.front();
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaEventSynchronize(e->tl_spec[r.run % abg_engine::TL_RUNS][1]));  // (a later record of it is a later run: also fine)
-    if (power) memcpy(power, d.spec_ring + (size_t)r.pos * e->N, sizeof(float) * e->N);
+    const unsigned char* src = nullptr;
+    MonitorQueue::Entry r{};
+    const int rc = monitor_pop(e, e->dev[dev].spec_q, e->tl_spec, &src, &r);
+    if (rc <= 0) return rc;
+    if (power) memcpy(power, src, sizeof(float) * e->N);
     if (batch_seq) *batch_seq = r.seq;
     if (n_frames) *n_frames = r.n_frames;
-    d.spec_ready.pop_front();
     return 1;
 }
 
@@ -1327,6 +1404,67 @@ int abg_debug_spectrum_time(abg_engine* e, float* ms) {
     if (e->run_index == 0 || !e->spec_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
     cudaSetDevice(e->cuda_dev);
     cudaEvent_t* ts = e->tl_spec[(e->run_index - 1) % abg_engine::TL_RUNS];
+    CU(cudaEventSynchronize(ts[1]));
+    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
+    return ABG_OK;
+}
+
+// ---- carrier frequency meter (definition in airband_b200.h) -----------------------------------------------------------
+int abg_carrier_configure(abg_engine* e, int dev, int on) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_carrier_configure: device %d out of range", dev);
+    if (on != 0 && on != 1) return fail(ABG_EINVAL, "abg_carrier_configure: on = %d is neither 0 nor 1", on);
+    Device& d = e->dev[dev];
+    if ((on == 1) == d.car_on) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream));  // an enqueued meter kernel may still read the device table
+    if (on) {
+        if (!e->tl_car[0][0])
+            for (auto& row : e->tl_car)
+                for (auto& ev : row) CU(cudaEventCreate(&ev));
+        if (!d.car_q.alloc(e->nbmax + 2, sizeof(float) * 3 * (size_t)std::max(d.C, 1))) return fail(ABG_ENOMEM, "Out of page-locked host memory for the carrier meter ring");
+    }
+    d.car_on = on == 1;
+    // rebuild the launch's device list and its static table
+    e->car_devs.clear();
+    std::vector<CarCfg> cfgs;
+    for (int i = 0; i < (int)e->dev.size(); i++) {
+        const Device& x = e->dev[i];
+        if (!x.car_on) continue;
+        CarCfg c{};
+        CU(cudaHostGetDevicePointer((void**)&c.ring, x.car_q.ring, 0));
+        c.g0 = x.g0; c.n_channels = x.C; c.ring_cap = x.car_q.cap;
+        e->car_devs.push_back(i);
+        cfgs.push_back(c);
+    }
+    e->car_cfg.free();
+    e->h_car_run.assign(e->car_devs.size(), CarRun{});
+    if (cfgs.empty()) return ABG_OK;
+    if (e->car_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the carrier meter tables");
+    CU(cudaMemcpy(e->car_cfg.p, cfgs.data(), sizeof(CarCfg) * cfgs.size(), cudaMemcpyHostToDevice));
+    // upload_small writes whole 16-byte words: room for every device plus the rounding
+    if (!e->car_run.p && e->car_run.alloc(e->dev.size() + 2)) return fail(ABG_ENOMEM, "Out of device memory for the carrier meter tables");
+    return ABG_OK;
+}
+
+int abg_fetch_carrier(abg_engine* e, int dev, float* lag1, float* energy, uint64_t* batch_seq) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_carrier: device %d out of range", dev);
+    const unsigned char* src = nullptr;
+    MonitorQueue::Entry r{};
+    const int C = e->dev[dev].C;
+    const int rc = monitor_pop(e, e->dev[dev].car_q, e->tl_car, &src, &r);
+    if (rc <= 0) return rc;
+    if (lag1) memcpy(lag1, src, sizeof(float) * 2 * C);
+    if (energy) memcpy(energy, src + sizeof(float) * 2 * C, sizeof(float) * C);
+    if (batch_seq) *batch_seq = r.seq;
+    return 1;
+}
+
+int abg_debug_carrier_time(abg_engine* e, float* ms) {
+    if (!ms) return fail(ABG_EINVAL, "abg_debug_carrier_time: null argument");
+    *ms = 0.0f;
+    if (e->run_index == 0 || !e->car_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    cudaEvent_t* ts = e->tl_car[(e->run_index - 1) % abg_engine::TL_RUNS];
     CU(cudaEventSynchronize(ts[1]));
     CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
     return ABG_OK;

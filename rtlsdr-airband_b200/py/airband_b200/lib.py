@@ -24,6 +24,7 @@ SYMBOLS = [
     "abg_resident_load", "abg_run_resident", "abg_set_stream", "abg_launch_count", "abg_mixers_configure",
     "abg_fetch_mixer_batch", "abg_mixer_device_buffers", "abg_debug_frame", "abg_last_run_times", "abg_debug_timeline", "abg_scan_configure", "abg_scan_select", "abg_host_register", "abg_host_unregister", "abg_ingest_sync", "abg_fft_path", "abg_debug_tc_table", "abg_debug_inject_wavein", "abg_debug_k1tc_trace", "abg_debug_k2_stats",
     "abg_debug_run_outputs", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
+    "abg_carrier_configure", "abg_fetch_carrier", "abg_debug_carrier_time",
 ]
 
 
@@ -100,6 +101,9 @@ def load():
     L.abg_fetch_spectrum.restype = i
     L.abg_fetch_spectrum.argtypes = [vp, i, vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
     L.abg_debug_spectrum_time.restype, L.abg_debug_spectrum_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_carrier_configure.restype, L.abg_carrier_configure.argtypes = i, [vp, i, i]
+    L.abg_fetch_carrier.restype, L.abg_fetch_carrier.argtypes = i, [vp, i, vp, vp, C.POINTER(C.c_uint64)]
+    L.abg_debug_carrier_time.restype, L.abg_debug_carrier_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -276,6 +280,29 @@ class Engine:
         self._chk(self.L.abg_debug_spectrum_time(self.h, C.byref(ms)))
         return float(ms.value)
 
+    # ---- carrier frequency meter ---------------------------------------------------------------------------------
+    def carrier_configure(self, dev: int, on: bool) -> None:
+        """Lag-one correlation and energy of every channel's bin per batch (off by default); applies to batches enqueued
+        by later runs.  `carrier_offset_hz` turns a reading into the carrier's frequency error."""
+        self._chk(self.L.abg_carrier_configure(self.h, dev, int(on)))
+
+    def fetch_carrier(self, dev: int) -> Optional[Tuple[np.ndarray, np.ndarray, int]]:
+        """Oldest unfetched meter reading of a device: (lag1 complex64[C], energy float32[C], batch_seq), or None.  Lossy:
+        at most max_batches_per_run + 2 are kept per device."""
+        Cn = len(self.cfg.devices[dev].channels) if 0 <= dev < len(self.cfg.devices) else 0  # (a bad index: the C call reports it)
+        lag1 = np.empty(2 * Cn, np.float32)
+        energy = np.empty(Cn, np.float32)
+        seq = C.c_uint64(0)
+        if not self._chk(self.L.abg_fetch_carrier(self.h, dev, _ptr(lag1), _ptr(energy), C.byref(seq))):
+            return None
+        return lag1.view(np.complex64), energy, int(seq.value)
+
+    def carrier_time(self) -> float:
+        """ms of the carrier meter kernel in the most recent run (CUDA events on the K1 stream); 0 if it metered nothing."""
+        ms = C.c_float(0.0)
+        self._chk(self.L.abg_debug_carrier_time(self.h, C.byref(ms)))
+        return float(ms.value)
+
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
         """mixers[m] = [(dev, chan, ampfactor, balance), ...]"""
@@ -331,6 +358,15 @@ def spectrum_dbfs(power: np.ndarray, fft_size: int) -> np.ndarray:
     with np.errstate(divide="ignore"):
         db = f32(20.0) * np.log10(level / f32(fft_size)) + offset
     return np.minimum(f32(0.0), db.astype(np.float32))
+
+
+def carrier_offset_hz(lag1, channel_offset_hz, sample_rate: float, hop: int) -> np.ndarray:
+    """Carrier frequency error in Hz relative to the configured channel from a carrier meter reading (definition in
+    airband_b200.h): wrap(arg(R) / (2 pi) - channel_offset_hz * hop / sample_rate) * sample_rate / hop, wrapped to
+    [-0.5, 0.5) frames, i.e. unambiguous within +-sample_rate / (2 hop).  channel_offset_hz = freq - centerfreq of the
+    channel (or of the scan entry the batch used); hop = abg_hop() / Config.hop(dev).  Arrays broadcast."""
+    cyc = np.angle(np.asarray(lag1, np.complex128)) / (2.0 * np.pi) - np.asarray(channel_offset_hz, np.float64) * hop / sample_rate
+    return (cyc - np.floor(cyc + 0.5)) * sample_rate / hop
 
 
 TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "acc_regs", "smem_bytes", "halo", "consumer_warpgroups")
