@@ -274,6 +274,52 @@ ABG_API int abg_fetch_carrier(abg_engine* e, int dev, float* lag1, float* energy
  * (0 if that run metered nothing).  Waits for it. */
 ABG_API int abg_debug_carrier_time(abg_engine* e, float* ms);
 
+/* Input level meter (not part of the reference surface: it shows how a device's gain sits in its ADC's range while the
+ * engine holds the SDR, which rtl_test or an SDR program's IQ histogram would otherwise need the dongle for).  For a device
+ * with the meter on, batch b (numbered as for the band spectrum) covers the n = WAVE_BATCH * hop complex samples
+ * s in [s0, s0 + n), s0 = (AGC_EXTRA + b*WAVE_BATCH) * hop, hop = abg_hop(): the first hop samples of each of the batch's
+ * frames.  Consecutive batches tile the stream after its first AGC_EXTRA * hop samples; no sample counts twice, and a
+ * reading depends on its batch only, never on how batches are grouped into runs or on push sizes.
+ * For each component k (0 = I, 1 = Q) of each sample the level v is the reference's conversion before the window
+ * (src/rtl_airband.cpp:316-324,402-455), in float32, rounded to nearest, no contraction:
+ *     U8: (c - 127.5f) / 127.5f     S8: c / 128.0f     S16: (1.0f / fullscale) * (float)x     F32: (1.0f / fullscale) * x
+ * and per batch
+ *     hist[k][i] = number of components with clamp(floor((v + 1.0f) * 128.0f), 0, 255) == i      (float32)
+ *     peak[k]    = max |v|                                                                            (float32)
+ *     sum[k] = sum v,   sum_sq[k] = sum v^2,   sum_iq = sum v_I * v_Q                                 (double)
+ * For U8 and S8 every ADC code has a bin of its own (U8: bin = code, S8: bin = code + 128), so hist is the code histogram
+ * and hist[k][0] + hist[k][255] counts the components at the ends of the ADC's range (U8 codes 0 and 255, S8 -128 and
+ * 127).  S16 and F32 bins are 1/128 of full scale wide: only the 8-bit formats give a per-code histogram; the end bins
+ * hold the outer 1/128 of the range and every level beyond full scale, and peak shows how far beyond it went.
+ * The sums of the integer formats are exact integer sums of the codes, converted once: they are the sums of the exact
+ * levels (2c - 255) / 255 (U8), c / 128 (S8) and x * (double)(1.0f / fullscale) (S16), before the float32 rounding of v.
+ * F32 sums add the float32 v in double, in a fixed order.  Every field is bitwise reproducible.
+ * Computed on the GPU by one extra kernel per run on the K1 stream, after K1 (and after the band spectrum and the carrier
+ * meter when those are on); it re-reads the device's raw bytes, K2 does not wait for it.  With every device off (the
+ * default) nothing is launched, allocated or copied.  Resident runs (abg_run_resident) compute readings but queue none;
+ * batches fed through abg_debug_inject_wavein have no samples and produce none. */
+typedef struct abg_input_levels {
+    uint64_t batch_seq;   /* as for abg_fetch_spectrum */
+    uint64_t n_samples;   /* complex samples, WAVE_BATCH * hop */
+    double sum[2];        /* [I, Q] */
+    double sum_sq[2];
+    double sum_iq;
+    float peak[2];
+    uint32_t hist[2][256];
+} abg_input_levels;
+/* abg_input_meter_configure: on = 1 / 0 switches the meter on / off for batches enqueued by later abg_run /
+ * abg_run_resident calls.  ABG_ERANGE for a bad device, ABG_EINVAL for any other value of on.  Waits for the engine's K1
+ * stream. */
+ABG_API int abg_input_meter_configure(abg_engine* e, int dev, int on);
+/* Pop the oldest unfetched reading of a device into *out.  Returns 1 if one was popped, 0 if none is ready, < 0 on error;
+ * waits for the run that computed it.  The queue is lossy exactly like the spectrum's: max_batches_per_run + 2 readings per
+ * device, the oldest overwritten first; the meter never holds a result slot or causes ABG_EOVERFLOW, and readings already
+ * queued stay fetchable after the meter is switched off. */
+ABG_API int abg_fetch_input_levels(abg_engine* e, int dev, abg_input_levels* out);
+/* Measurement aid: device time of the meter kernel of the most recent run, from CUDA events around it on the K1 stream
+ * (0 if that run metered nothing).  Waits for it. */
+ABG_API int abg_debug_input_meter_time(abg_engine* e, float* ms);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

@@ -202,6 +202,30 @@ struct CarArgs {
 cudaError_t abg_launch_carrier(const CarArgs& a, int n_devices, int max_items, cudaStream_t s);
 int abg_carrier_items(int n_channels);  // work items per batch of a device
 
+// input level meter (input_meter.cu): see abg_input_meter_configure in include/airband_b200.h
+struct InmCfg {  // per metered device; written by abg_input_meter_configure
+    unsigned char* ring;   // device view of the page-locked result ring [ring_cap] of abg_input_levels
+    uint32_t* hist;        // [max_batches_per_run][2][256] histogram of each batch of the run; zero between launches
+    int32_t* counter;      // [max_batches_per_run] chunks finished per batch; zero between launches
+    long long* partial;    // [max_batches_per_run][n_chunks][ABG_INM_PARTIAL] chunk sums (int64, or double for F32)
+    int32_t sfmt, hop_bytes, n_chunks, ring_cap;
+    float scale;           // 1.0f / fullscale (S16, F32)
+};
+#define ABG_INM_PARTIAL 6  // per chunk: sum[2], sum_sq[2], sum_iq, then peak[2] as two float bit patterns
+struct InmRun {  // per metered device; uploaded with every run
+    const unsigned char* raw;
+    unsigned long long first_byte;  // first byte of the run's first batch
+    int32_t n_batches;              // batches of this run (0 = none)
+    int32_t ring_pos0;              // ring entry of the run's first batch; < 0: resident run, the ring is left alone
+};
+struct InmArgs {
+    const InmCfg* cfg;  // [metered devices]
+    const InmRun* run;
+    int wave_batch;
+};
+cudaError_t abg_launch_input_meter(const InmArgs& a, int n_devices, int max_items, cudaStream_t s);
+int abg_input_meter_chunks(int batch_bytes);  // work items per batch of a device
+
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B
     int lanes_per_warp;       // channels handled by one warp of K2: 1, 2, 4, 8, 16 or 32

@@ -167,10 +167,10 @@ struct DevBuf {
     }
 };
 
-// Result queue of one device's batch monitor (band spectrum, carrier meter).  The monitor's kernel writes the result of
-// every batch straight into a page-locked, mapped ring of `cap` = max_batches_per_run + 2 entries; the host keeps the
-// unfetched entries, oldest first.  Lossy by design: queueing a run drops the oldest unfetched entries beyond the ring's
-// size (gaps show in their batch_seq), so a monitor never holds a result slot or causes ABG_EOVERFLOW.
+// Result queue of one device's batch monitor (band spectrum, carrier meter, input level meter).  The monitor's kernel
+// writes the result of every batch straight into a page-locked, mapped ring of `cap` = max_batches_per_run + 2 entries;
+// the host keeps the unfetched entries, oldest first.  Lossy by design: queueing a run drops the oldest unfetched entries
+// beyond the ring's size (gaps show in their batch_seq), so a monitor never holds a result slot or causes ABG_EOVERFLOW.
 struct MonitorQueue {
     struct Entry {
         int pos;           // ring entry
@@ -231,6 +231,11 @@ struct Device {
     // carrier frequency meter (abg_carrier_configure); nothing is allocated until it is first switched on
     bool car_on = false;
     MonitorQueue car_q;          // lag1 float[C][2], then energy float[C] per entry
+    // input level meter (abg_input_meter_configure); nothing is allocated until it is first switched on
+    bool inm_on = false;
+    int inm_chunks = 0;
+    void* inm_work = nullptr;    // device: histograms uint32[nbmax][2][256], counters int32[nbmax], chunk sums int64[nbmax][inm_chunks][ABG_INM_PARTIAL]; kept once allocated
+    MonitorQueue inm_q;          // abg_input_levels per entry
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -371,7 +376,8 @@ struct abg_engine {
     DevBuf<SpecCfg> spec_cfg;                // [spec_devs.size()]
     DevBuf<SpecRun> spec_run;                // room for every device
     std::vector<SpecRun> h_spec_run;
-    cudaEvent_t ev_spec[2] = {nullptr, nullptr};  // after the spectrum kernel of the latest run of each parity (it reads raw[])
+    cudaEvent_t ev_raw[2] = {nullptr, nullptr};   // after the last kernel that read raw[] (K1 aside: the band spectrum, the
+                                                  // input meter) of the latest run of each parity that ran one
     cudaEvent_t tl_spec[TL_RUNS][2] = {};    // spectrum kernel start / end of the last TL_RUNS runs
     bool spec_ran[TL_RUNS] = {};
     // carrier frequency meter
@@ -381,6 +387,13 @@ struct abg_engine {
     std::vector<CarRun> h_car_run;
     cudaEvent_t tl_car[TL_RUNS][2] = {};     // meter kernel start / end of the last TL_RUNS runs
     bool car_ran[TL_RUNS] = {};
+    // input level meter
+    std::vector<int> inm_devs;               // metered devices in launch order (grid.y of the meter kernel)
+    DevBuf<InmCfg> inm_cfg;                  // [inm_devs.size()]
+    DevBuf<InmRun> inm_run;                  // room for every device
+    std::vector<InmRun> h_inm_run;
+    cudaEvent_t tl_inm[TL_RUNS][2] = {};     // meter kernel start / end of the last TL_RUNS runs
+    bool inm_ran[TL_RUNS] = {};
     // mixers (reference src/mixer.cpp)
     int n_mixers = 0;
     DevBuf<int32_t> mix_offsets;
@@ -416,15 +429,21 @@ void engine_free(abg_engine* e) {
         if (d.res) cudaFree(d.res);
         if (d.spec) cudaFree(d.spec);
         if (d.spec_work) cudaFree(d.spec_work);
+        if (d.inm_work) cudaFree(d.inm_work);
         d.spec_q.release();
         d.car_q.release();
+        d.inm_q.release();
     }
     e->spec_cfg.free(); e->spec_run.free();
     e->car_cfg.free(); e->car_run.free();
+    e->inm_cfg.free(); e->inm_run.free();
     for (auto& row : e->tl_spec)
         for (auto& ev : row)
             if (ev) cudaEventDestroy(ev);
     for (auto& row : e->tl_car)
+        for (auto& ev : row)
+            if (ev) cudaEventDestroy(ev);
+    for (auto& row : e->tl_inm)
         for (auto& ev : row)
             if (ev) cudaEventDestroy(ev);
     for (auto& g : e->groups) {
@@ -453,7 +472,7 @@ void engine_free(abg_engine* e) {
     for (int k = 0; k < 2; k++) {
         if (e->ev_k1[k]) cudaEventDestroy(e->ev_k1[k]);
         if (e->ev_k2[k]) cudaEventDestroy(e->ev_k2[k]);
-        if (e->ev_spec[k]) cudaEventDestroy(e->ev_spec[k]);
+        if (e->ev_raw[k]) cudaEventDestroy(e->ev_raw[k]);
     }
     if (e->stream_b) cudaStreamDestroy(e->stream_b);
     if (e->stream_c) {
@@ -974,7 +993,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             if (ers != cudaSuccess) return fail(ABG_ECUDA, "spectrum launch failed: %s", cudaGetErrorString(ers));
             e->launches++;
             CU(cudaEventRecord(ts[1], sa));
-            CU(cudaEventRecord(e->ev_spec[cur], sa));
+            CU(cudaEventRecord(e->ev_raw[cur], sa));
             e->spec_ran[ri % abg_engine::TL_RUNS] = true;
         }
     }
@@ -1004,6 +1023,40 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             e->launches++;
             CU(cudaEventRecord(ts[1], sa));
             e->car_ran[ri % abg_engine::TL_RUNS] = true;
+        }
+    }
+    // ---- input level meter of the metered devices (stream A: after K1, the spectrum and the carrier meter; reads the
+    // raw bytes K1 read, so abg_push's compaction waits for it through ev_raw) ----
+    e->inm_ran[ri % abg_engine::TL_RUNS] = false;
+    if (!skip_k1 && !e->inm_devs.empty()) {
+        int max_items = 0;
+        for (size_t m = 0; m < e->inm_devs.size(); m++) {
+            Device& d = e->dev[e->inm_devs[m]];
+            const int n = nb[e->inm_devs[m]];
+            InmRun& r = e->h_inm_run[m];
+            const bool primed = resident ? d.res_primed : d.primed;
+            r.raw = resident ? d.res : d.raw[d.cur];
+            // the same first byte as the spectrum's frame j = 0 of the run's first batch
+            r.first_byte = resident ? (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes
+                                    : (unsigned long long)d.consumed + (primed ? 0ull : (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes);
+            r.n_batches = n;
+            r.ring_pos0 = queue_outputs && n > 0 ? d.inm_q.queue(n, d.batch_seq, ri, 0) : -1;
+            max_items = std::max(max_items, n * d.inm_chunks);
+        }
+        if (max_items > 0) {
+            const int nl = upload_small(e->inm_run.p, e->h_inm_run.data(), sizeof(InmRun) * e->inm_devs.size(), sa);
+            if (nl < 0) return fail(ABG_ECUDA, "input meter parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+            e->launches += (uint64_t)nl;
+            InmArgs A{};
+            A.cfg = e->inm_cfg.p; A.run = e->inm_run.p; A.wave_batch = B;
+            cudaEvent_t* ts = e->tl_inm[ri % abg_engine::TL_RUNS];
+            CU(cudaEventRecord(ts[0], sa));
+            cudaError_t eri = abg_launch_input_meter(A, (int)e->inm_devs.size(), max_items, sa);
+            if (eri != cudaSuccess) return fail(ABG_ECUDA, "input meter launch failed: %s", cudaGetErrorString(eri));
+            e->launches++;
+            CU(cudaEventRecord(ts[1], sa));
+            CU(cudaEventRecord(e->ev_raw[cur], sa));
+            e->inm_ran[ri % abg_engine::TL_RUNS] = true;
         }
     }
     // ---- K2 (stream B, after this run's K1; overlaps the next run's K1) ----
@@ -1151,15 +1204,15 @@ int abg_push(abg_engine* e, int dev, const void* iq, size_t nbytes) {
         }
         // the destination buffer was last read by a K1 launched before the previous compaction: with at least one run since
         // then that is run_index-2 or older, so the copy overlaps the K1 that is reading the current buffer right now
-        // (the band spectrum kernel reads the same bytes right after that K1)
+        // (the band spectrum and the input meter read the same bytes right after that K1: ev_raw follows the last of them)
         if (d.runs_since_compaction >= 1) {
             if (e->run_index >= 2) {
                 CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 2) & 1], 0));
-                if (e->ev_spec[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_spec[(e->run_index - 2) & 1], 0));
+                if (e->ev_raw[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_raw[(e->run_index - 2) & 1], 0));
             }
         } else if (e->run_index >= 1) {
             CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 1) & 1], 0));
-            if (e->ev_spec[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_spec[(e->run_index - 1) & 1], 0));
+            if (e->ev_raw[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_raw[(e->run_index - 1) & 1], 0));
         }
         d.runs_since_compaction = 0;
         CU(cudaMemcpyAsync(d.raw[d.cur ^ 1], d.raw[d.cur] + keep_from, rem, cudaMemcpyDeviceToDevice, e->stream_c));
@@ -1316,6 +1369,13 @@ int abg_fft_path(const abg_engine* e, int dev) {
     return g.use_tc ? 3 : (g.pruned ? 2 : 1);
 }
 
+// The monitors that read raw[] after K1 (band spectrum, input meter) record ev_raw, which abg_push's compaction waits for.
+static int create_raw_events(abg_engine* e) {
+    if (e->ev_raw[0]) return ABG_OK;
+    for (int k = 0; k < 2; k++) CU(cudaEventCreateWithFlags(&e->ev_raw[k], cudaEventDisableTiming));
+    return ABG_OK;
+}
+
 // ---- band spectrum monitor (definition in airband_b200.h) -------------------------------------------------------------
 int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_spectrum_configure: device %d out of range", dev);
@@ -1329,11 +1389,11 @@ int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
     d.spec_work = nullptr;
     d.spec_stride = d.spec_n_sel = d.spec_chunks = 0;
     if (frame_stride > 0) {
-        if (!e->ev_spec[0]) {
-            for (int k = 0; k < 2; k++) CU(cudaEventCreateWithFlags(&e->ev_spec[k], cudaEventDisableTiming));
+        if (!e->tl_spec[0][0]) {
             for (auto& row : e->tl_spec)
                 for (auto& ev : row) CU(cudaEventCreate(&ev));
         }
+        if (create_raw_events(e) != ABG_OK) return ABG_ECUDA;
         if (!d.spec_q.alloc(nbmax + 2, sizeof(float) * N)) return fail(ABG_ENOMEM, "Out of page-locked host memory for the spectrum ring");
         const int n_sel = (B + frame_stride - 1) / frame_stride;
         const int chunks = (n_sel + ABG_SPEC_FPC - 1) / ABG_SPEC_FPC;
@@ -1470,6 +1530,86 @@ int abg_debug_carrier_time(abg_engine* e, float* ms) {
     return ABG_OK;
 }
 
+// ---- input level meter (definition in airband_b200.h) -----------------------------------------------------------------
+int abg_input_meter_configure(abg_engine* e, int dev, int on) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_input_meter_configure: device %d out of range", dev);
+    if (on != 0 && on != 1) return fail(ABG_EINVAL, "abg_input_meter_configure: on = %d is neither 0 nor 1", on);
+    Device& d = e->dev[dev];
+    if ((on == 1) == d.inm_on) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream));  // an enqueued meter kernel may still read the device table
+    const int nbmax = e->nbmax;
+    const int chunks = abg_input_meter_chunks(e->B * d.hop_bytes);
+    const size_t hist_bytes = sizeof(uint32_t) * 512 * (size_t)nbmax, counter_bytes = sizeof(int32_t) * (size_t)nbmax;
+    const size_t part_off = (hist_bytes + counter_bytes + 15) & ~(size_t)15;
+    if (on) {
+        if (!e->tl_inm[0][0])
+            for (auto& row : e->tl_inm)
+                for (auto& ev : row) CU(cudaEventCreate(&ev));
+        if (create_raw_events(e) != ABG_OK) return ABG_ECUDA;
+        if (!d.inm_q.alloc(nbmax + 2, sizeof(abg_input_levels))) return fail(ABG_ENOMEM, "Out of page-locked host memory for the input meter ring");
+        if (!d.inm_work) {
+            // histograms and counters start at zero; every launch leaves them at zero again
+            if (cudaMalloc(&d.inm_work, part_off + sizeof(long long) * ABG_INM_PARTIAL * (size_t)nbmax * chunks) != cudaSuccess) {
+                d.inm_work = nullptr;
+                return fail(ABG_ENOMEM, "Out of device memory for the input meter of device %d", dev);
+            }
+            CU(cudaMemset(d.inm_work, 0, part_off));
+        }
+        d.inm_chunks = chunks;
+    }
+    d.inm_on = on == 1;
+    // rebuild the launch's device list and its static table
+    e->inm_devs.clear();
+    std::vector<InmCfg> cfgs;
+    for (int i = 0; i < (int)e->dev.size(); i++) {
+        const Device& x = e->dev[i];
+        if (!x.inm_on) continue;
+        InmCfg c{};
+        CU(cudaHostGetDevicePointer((void**)&c.ring, x.inm_q.ring, 0));
+        char* w = static_cast<char*>(x.inm_work);
+        c.hist = reinterpret_cast<uint32_t*>(w);
+        c.counter = reinterpret_cast<int32_t*>(w + hist_bytes);
+        c.partial = reinterpret_cast<long long*>(w + part_off);
+        c.sfmt = x.sfmt; c.hop_bytes = x.hop_bytes; c.n_chunks = x.inm_chunks; c.ring_cap = x.inm_q.cap;
+        c.scale = 1.0f / x.fullscale;
+        e->inm_devs.push_back(i);
+        cfgs.push_back(c);
+    }
+    e->inm_cfg.free();
+    e->h_inm_run.assign(e->inm_devs.size(), InmRun{});
+    if (cfgs.empty()) return ABG_OK;
+    if (e->inm_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the input meter tables");
+    CU(cudaMemcpy(e->inm_cfg.p, cfgs.data(), sizeof(InmCfg) * cfgs.size(), cudaMemcpyHostToDevice));
+    // upload_small writes whole 16-byte words: room for every device plus the rounding
+    if (!e->inm_run.p && e->inm_run.alloc(e->dev.size() + 1)) return fail(ABG_ENOMEM, "Out of device memory for the input meter tables");
+    return ABG_OK;
+}
+
+int abg_fetch_input_levels(abg_engine* e, int dev, abg_input_levels* out) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_input_levels: device %d out of range", dev);
+    const unsigned char* src = nullptr;
+    MonitorQueue::Entry r{};
+    const int rc = monitor_pop(e, e->dev[dev].inm_q, e->tl_inm, &src, &r);
+    if (rc <= 0) return rc;
+    if (out) {
+        memcpy(out, src, sizeof(abg_input_levels));
+        out->batch_seq = r.seq;
+    }
+    return 1;
+}
+
+int abg_debug_input_meter_time(abg_engine* e, float* ms) {
+    if (!ms) return fail(ABG_EINVAL, "abg_debug_input_meter_time: null argument");
+    *ms = 0.0f;
+    if (e->run_index == 0 || !e->inm_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    cudaEvent_t* ts = e->tl_inm[(e->run_index - 1) % abg_engine::TL_RUNS];
+    CU(cudaEventSynchronize(ts[1]));
+    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
+    return ABG_OK;
+}
+
 // ---- scan mode -------------------------------------------------------------------------------------------------------
 static ScanView scan_view(abg_engine* e) {
     ScanView v;
@@ -1581,12 +1721,16 @@ int abg_resident_load(abg_engine* e, int dev, const void* iq, size_t nbytes) {
     Device& d = e->dev[dev];
     const size_t need = (size_t)(e->nbmax * e->B + ABG_AGC_EXTRA - 1) * d.hop_bytes + (size_t)e->N * d.bpc;
     if (nbytes < need) return fail(ABG_EINVAL, "abg_resident_load: need at least %zu bytes for %d batches, got %zu", need, e->nbmax, nbytes);
+    // The input meter reads the first hop samples of every frame of a batch, up to (AGC_EXTRA + nbmax*B) * hop_bytes:
+    // past `need` when hop > fft_size.  The tail it reads there is zeros (resident runs queue no readings).
+    const size_t meter_end = (size_t)(e->nbmax * e->B + ABG_AGC_EXTRA) * d.hop_bytes;
+    const size_t alloc = std::max(need, meter_end) + 256;
     cudaSetDevice(e->cuda_dev);
     if (d.res) cudaFree(d.res);
     d.res = nullptr;
-    if (cudaMalloc((void**)&d.res, need + 256) != cudaSuccess) return fail(ABG_ENOMEM, "Out of device memory for the resident stream");
+    if (cudaMalloc((void**)&d.res, alloc) != cudaSuccess) return fail(ABG_ENOMEM, "Out of device memory for the resident stream");
     d.res_bytes = need;
-    CU(cudaMemsetAsync(d.res + need, 0, 256, e->stream));
+    CU(cudaMemsetAsync(d.res + need, 0, alloc - need, e->stream));
     CU(cudaMemcpyAsync(d.res, iq, need, cudaMemcpyHostToDevice, e->stream));
     CU(cudaStreamSynchronize(e->stream));
     return ABG_OK;

@@ -25,6 +25,7 @@ SYMBOLS = [
     "abg_fetch_mixer_batch", "abg_mixer_device_buffers", "abg_debug_frame", "abg_last_run_times", "abg_debug_timeline", "abg_scan_configure", "abg_scan_select", "abg_host_register", "abg_host_unregister", "abg_ingest_sync", "abg_fft_path", "abg_debug_tc_table", "abg_debug_inject_wavein", "abg_debug_k1tc_trace", "abg_debug_k2_stats",
     "abg_debug_run_outputs", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
     "abg_carrier_configure", "abg_fetch_carrier", "abg_debug_carrier_time",
+    "abg_input_meter_configure", "abg_fetch_input_levels", "abg_debug_input_meter_time",
 ]
 
 
@@ -40,6 +41,19 @@ class COptions(C.Structure):
 
 class CMixerInput(C.Structure):
     _fields_ = [("dev", C.c_int32), ("chan", C.c_int32), ("ampfactor", C.c_float), ("balance", C.c_float)]
+
+
+class CInputLevels(C.Structure):
+    """abg_input_levels: one input level meter reading (definition in airband_b200.h)."""
+    _fields_ = [
+        ("batch_seq", C.c_uint64),
+        ("n_samples", C.c_uint64),
+        ("sum", C.c_double * 2),
+        ("sum_sq", C.c_double * 2),
+        ("sum_iq", C.c_double),
+        ("peak", C.c_float * 2),
+        ("hist", (C.c_uint32 * 256) * 2),
+    ]
 
 
 class AbgError(RuntimeError):
@@ -104,6 +118,9 @@ def load():
     L.abg_carrier_configure.restype, L.abg_carrier_configure.argtypes = i, [vp, i, i]
     L.abg_fetch_carrier.restype, L.abg_fetch_carrier.argtypes = i, [vp, i, vp, vp, C.POINTER(C.c_uint64)]
     L.abg_debug_carrier_time.restype, L.abg_debug_carrier_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_input_meter_configure.restype, L.abg_input_meter_configure.argtypes = i, [vp, i, i]
+    L.abg_fetch_input_levels.restype, L.abg_fetch_input_levels.argtypes = i, [vp, i, C.POINTER(CInputLevels)]
+    L.abg_debug_input_meter_time.restype, L.abg_debug_input_meter_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -303,6 +320,29 @@ class Engine:
         self._chk(self.L.abg_debug_carrier_time(self.h, C.byref(ms)))
         return float(ms.value)
 
+    # ---- input level meter ---------------------------------------------------------------------------------------
+    def input_meter_configure(self, dev: int, on: bool) -> None:
+        """Histogram, peak and moments of a device's I and Q input levels per batch (off by default); applies to batches
+        enqueued by later runs.  `input_levels` turns a reading into DC offset, dBFS, clipping and I/Q balance."""
+        self._chk(self.L.abg_input_meter_configure(self.h, dev, int(on)))
+
+    def fetch_input_levels(self, dev: int) -> Optional[dict]:
+        """Oldest unfetched reading of a device, or None: a dict of batch_seq, n_samples (int), sum, sum_sq (float64[2]),
+        sum_iq (float), peak (float32[2]) and hist (uint32[2, 256]).  Lossy: at most max_batches_per_run + 2 are kept per
+        device."""
+        r = CInputLevels()
+        if not self._chk(self.L.abg_fetch_input_levels(self.h, dev, C.byref(r))):
+            return None
+        return dict(batch_seq=int(r.batch_seq), n_samples=int(r.n_samples), sum=np.array(r.sum, np.float64),
+                    sum_sq=np.array(r.sum_sq, np.float64), sum_iq=float(r.sum_iq), peak=np.array(r.peak, np.float32),
+                    hist=np.ctypeslib.as_array(r.hist).astype(np.uint32).reshape(2, 256))
+
+    def input_meter_time(self) -> float:
+        """ms of the input meter kernel in the most recent run (CUDA events on the K1 stream); 0 if it metered nothing."""
+        ms = C.c_float(0.0)
+        self._chk(self.L.abg_debug_input_meter_time(self.h, C.byref(ms)))
+        return float(ms.value)
+
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
         """mixers[m] = [(dev, chan, ampfactor, balance), ...]"""
@@ -367,6 +407,32 @@ def carrier_offset_hz(lag1, channel_offset_hz, sample_rate: float, hop: int) -> 
     channel (or of the scan entry the batch used); hop = abg_hop() / Config.hop(dev).  Arrays broadcast."""
     cyc = np.angle(np.asarray(lag1, np.complex128)) / (2.0 * np.pi) - np.asarray(channel_offset_hz, np.float64) * hop / sample_rate
     return (cyc - np.floor(cyc + 0.5)) * sample_rate / hop
+
+
+def input_levels(reading: dict) -> dict:
+    """What an operator reads off an input level meter reading (Engine.fetch_input_levels; definition in airband_b200.h),
+    per component k = 0 (I), 1 (Q) where an array:
+      dc_offset           mean v_k, in full scale
+      mean_square_dbfs    10 log10(mean v_k^2); a full-scale sine reads -3.01 dBFS, and the DC offset counts
+      full_scale_fraction (hist[k][0] + hist[k][255]) / n: the components at the ends of the range (8-bit: clipped codes)
+      codes_in_use        non-empty bins (8-bit: distinct ADC codes)
+      imbalance_db        10 log10(var_I / var_Q)
+      phase_skew_deg      asin(cov_IQ / sqrt(var_I var_Q)) in degrees; I = cos, Q = sin(. + phi) reads phi
+    Variances and the covariance are about the means."""
+    n = float(reading["n_samples"])
+    s = np.asarray(reading["sum"], np.float64)
+    ss = np.asarray(reading["sum_sq"], np.float64)
+    h = np.asarray(reading["hist"]).reshape(2, 256)
+    mean = s / n
+    ms = ss / n
+    var = ms - mean * mean
+    cov = float(reading["sum_iq"]) / n - mean[0] * mean[1]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        ms_db = 10.0 * np.log10(ms)
+        imb = float(10.0 * np.log10(var[0] / var[1]))
+        skew = float(np.degrees(np.arcsin(np.clip(cov / np.sqrt(var[0] * var[1]), -1.0, 1.0))))
+    return dict(dc_offset=mean, mean_square_dbfs=ms_db, full_scale_fraction=(h[:, 0] + h[:, 255]).astype(np.float64) / n,
+                codes_in_use=np.count_nonzero(h, axis=1), imbalance_db=imb, phase_skew_deg=skew)
 
 
 TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "acc_regs", "smem_bytes", "halo", "consumer_warpgroups")
