@@ -347,6 +347,12 @@ ABG_API int abg_debug_frame(abg_engine* e, int dev, const void* iq_frame, float*
 /* The most recent run's results as the device holds them (resident runs export nothing): wout float[Gp][P] channel-major
  * audio ([0, AGC_EXTRA) is already the next run's look-back), axc[max_batches_per_run][Gp]; dims[4] = {G, Gp, P, nb}. */
 ABG_API int abg_debug_run_outputs(abg_engine* e, int32_t* dims, float* wout, unsigned char* axc);
+/* What K1 of the most recent run stored (resident runs included), before any demodulation: rows [AGC_EXTRA, AGC_EXTRA + rows)
+ * of its time-major output buffers, win float[rows][Gp] = |X[bin]| (channel_t.wavein) and iqin float[rows][Gp][2] = X[bin]
+ * (channel_t.iq_in); dims[4] = {G, Gp, rows, nb} with rows = max_batches_per_run * WAVE_BATCH.  Row j of a device that ran n
+ * batches is its frame AGC_EXTRA + (batches before the run) * WAVE_BATCH + j for j < n * WAVE_BATCH and stale beyond.  K2 never
+ * writes these rows, so closed-squelch stretches are visible here.  Waits for the run; either pointer may be NULL. */
+ABG_API int abg_debug_k1_outputs(abg_engine* e, int32_t* dims, float* win, float* iqin);
 /* Feed |X[bin]| values straight into the demodulation state machine of one device (K1 skipped): wavein[C][n_batches *
  * WAVE_BATCH] becomes channel_t.wavein[AGC_EXTRA ...]; results are fetched as usual.  For the ports of the reference's own
  * Squelch / CTCSS unit tests (reference src/test_squelch.cpp:51-281, src/test_ctcss.cpp:122-155).  The device must not be
@@ -359,8 +365,9 @@ ABG_API int abg_debug_k1tc_trace(long long* out);
 ABG_API int abg_debug_k2_stats(unsigned long long* out);
 /* Host-only: plan and coefficient table of the tensor-core K1 (fft_mode 3) for one device, as abg_create builds them
  * (window * twiddle quantised to `digits` signed 8-bit digits, in the shared-memory image the MMA reads).
- * plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups} (KBS = k-steps per
- * shared-memory stage at most, NSTB = stages in the ring); tab == NULL queries the plan only. */
+ * plan[14] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups, pps} (KBS = k-steps
+ * per column pair and shared-memory stage at most, NSTB = stages in the ring, pps = column pairs per stage at most);
+ * tab == NULL queries the plan only. */
 ABG_API int abg_debug_tc_table(int fft_size, int sfmt, int hop_bytes, float fullscale, int n_channels, const int32_t* bins, int digits,
                                int32_t* plan, signed char* tab, size_t tab_cap, long long* sq, double* cscale);
 

@@ -1862,13 +1862,13 @@ int abg_mixer_device_buffers(abg_engine* e, float** dev_sums, int32_t** dev_flag
 }
 
 // Host-only (no device needed): the tensor-core K1's plan and coefficient table for one device, exactly as abg_create
-// builds them.  plan[13] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups}.  tab may be null to
-// query the plan; otherwise tab_cap >= K*NC bytes and sq has C2p entries.
+// builds them.  plan[14] = {eligible, K, HC, S, NC, ND, C2p, KBS, NSTB, acc_regs, smem_bytes, halo, consumer_warpgroups, pps}.  tab may be
+// null to query the plan; otherwise tab_cap >= K*NC bytes and sq has C2p entries.
 int abg_debug_tc_table(int fft_size, int sfmt, int hop_bytes, float fullscale, int n_channels, const int32_t* bins, int digits, int32_t* plan,
                        signed char* tab, size_t tab_cap, long long* sq, double* cscale) {
     K1TcPlan p;
     abg_k1tc_plan(fft_size, sfmt, hop_bytes, n_channels, digits, &p);
-    const int32_t v[13] = {p.eligible, p.K, p.HC, p.S, p.NC, p.ND, p.C2p, p.KBS, p.NSTB, p.acc_regs, p.smem_bytes, p.halo, p.consumer_warpgroups};
+    const int32_t v[14] = {p.eligible, p.K, p.HC, p.S, p.NC, p.ND, p.C2p, p.KBS, p.NSTB, p.acc_regs, p.smem_bytes, p.halo, p.consumer_warpgroups, p.pps};
     if (plan) memcpy(plan, v, sizeof(v));
     if (!p.eligible) return fail(ABG_EINVAL, "abg_debug_tc_table: configuration not eligible for the tensor-core K1");
     if (!tab) return ABG_OK;
@@ -1924,6 +1924,24 @@ int abg_debug_run_outputs(abg_engine* e, int32_t* dims, float* wout, unsigned ch
     CU(cudaDeviceSynchronize());
     if (wout) CU(cudaMemcpy(wout, e->wout.p, sizeof(float) * (size_t)e->Gp * e->P, cudaMemcpyDeviceToHost));
     if (axc) CU(cudaMemcpy(axc, e->axc.p, (size_t)e->nbmax * e->Gp, cudaMemcpyDeviceToHost));
+    return ABG_OK;
+}
+
+// see airband_b200.h: rows [AGC_EXTRA, AGC_EXTRA + nbmax*B) of the win / iqin buffer the most recent run's K1 filled.  K2 of
+// that run only reads it; what K2 writes are the look-back rows [0, AGC_EXTRA) of the other buffer (k2_launch: win_next).
+int abg_debug_k1_outputs(abg_engine* e, int32_t* dims, float* win, float* iqin) {
+    const int rows = e->nbmax * e->B;
+    if (dims) {
+        dims[0] = e->G; dims[1] = e->Gp; dims[2] = rows; dims[3] = e->nbmax;
+    }
+    if (!win && !iqin) return ABG_OK;
+    if (e->run_index == 0) return fail(ABG_EINVAL, "abg_debug_k1_outputs: nothing has run yet");
+    int rc = abg_sync(e);
+    if (rc != ABG_OK) return rc;
+    const int cur = (int)((e->run_index - 1) & 1);
+    const size_t first = (size_t)ABG_AGC_EXTRA * e->Gp, n = (size_t)rows * e->Gp;
+    if (win) CU(cudaMemcpy(win, e->win[cur].p + first, sizeof(float) * n, cudaMemcpyDeviceToHost));
+    if (iqin) CU(cudaMemcpy(iqin, e->iqin[cur].p + first, sizeof(float2) * n, cudaMemcpyDeviceToHost));
     return ABG_OK;
 }
 

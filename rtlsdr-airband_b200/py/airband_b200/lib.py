@@ -23,7 +23,7 @@ SYMBOLS = [
     "abg_batches_available", "abg_run", "abg_sync", "abg_join", "abg_batches_ready", "abg_fetch_batch", "abg_fetch_batches", "abg_get_stats", "abg_set_bin",
     "abg_resident_load", "abg_run_resident", "abg_set_stream", "abg_launch_count", "abg_mixers_configure",
     "abg_fetch_mixer_batch", "abg_mixer_device_buffers", "abg_debug_frame", "abg_last_run_times", "abg_debug_timeline", "abg_scan_configure", "abg_scan_select", "abg_host_register", "abg_host_unregister", "abg_ingest_sync", "abg_fft_path", "abg_debug_tc_table", "abg_debug_inject_wavein", "abg_debug_k1tc_trace", "abg_debug_k2_stats",
-    "abg_debug_run_outputs", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
+    "abg_debug_run_outputs", "abg_debug_k1_outputs", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
     "abg_carrier_configure", "abg_fetch_carrier", "abg_debug_carrier_time",
     "abg_input_meter_configure", "abg_fetch_input_levels", "abg_debug_input_meter_time",
 ]
@@ -100,6 +100,7 @@ def load():
     L.abg_mixer_device_buffers.restype, L.abg_mixer_device_buffers.argtypes = i, [vp, C.POINTER(vp), C.POINTER(vp)]
     L.abg_debug_frame.restype, L.abg_debug_frame.argtypes = i, [vp, i, vp, vp]
     L.abg_debug_run_outputs.restype, L.abg_debug_run_outputs.argtypes = i, [vp, vp, vp, vp]
+    L.abg_debug_k1_outputs.restype, L.abg_debug_k1_outputs.argtypes = i, [vp, vp, vp, vp]
     L.abg_last_run_times.restype, L.abg_last_run_times.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_host_register.restype, L.abg_host_register.argtypes = i, [vp, C.c_size_t]
     L.abg_host_unregister.restype, L.abg_host_unregister.argtypes = i, [vp]
@@ -248,6 +249,18 @@ class Engine:
         axc = np.empty((nb, Gp), np.uint8)
         self._chk(self.L.abg_debug_run_outputs(self.h, _ptr(dims), _ptr(wout), _ptr(axc)))
         return wout[:G], axc[:, :G]
+
+    def k1_outputs(self):
+        """(win[rows, G] float32, iqin[rows, G] complex64) as K1 of the most recent run stored them, rows = max_batches_per_run *
+        WAVE_BATCH starting at the run's first batch (abg_debug_k1_outputs); a device's rows beyond its batches of that run are
+        stale."""
+        dims = np.zeros(4, np.int32)
+        self._chk(self.L.abg_debug_k1_outputs(self.h, _ptr(dims), None, None))
+        G, Gp, rows, _ = (int(x) for x in dims)
+        win = np.empty((rows, Gp), np.float32)
+        iqin = np.empty((rows, 2 * Gp), np.float32)
+        self._chk(self.L.abg_debug_k1_outputs(self.h, _ptr(dims), _ptr(win), _ptr(iqin)))
+        return win[:, :G], iqin.view(np.complex64)[:, :G]
 
     def set_stream(self, cuda_stream_ptr: int) -> None:
         self._chk(self.L.abg_set_stream(self.h, C.c_void_p(cuda_stream_ptr)))
@@ -435,19 +448,26 @@ def input_levels(reading: dict) -> dict:
                 codes_in_use=np.count_nonzero(h, axis=1), imbalance_db=imb, phase_skew_deg=skew)
 
 
-TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "acc_regs", "smem_bytes", "halo", "consumer_warpgroups")
+TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "acc_regs", "smem_bytes", "halo", "consumer_warpgroups", "pps")
+
+
+def tc_plan(fft_size: int, sfmt: int, hop_bytes: int, n_channels: int, digits: int = 4) -> dict:
+    """Host-only: the tensor-core K1's geometry for a launch group whose largest device has n_channels channels
+    (abg_debug_tc_table with no table); plan["eligible"] == 0 when the group would use the FP32 kernels."""
+    plan = np.zeros(len(TC_PLAN_FIELDS), np.int32)
+    load().abg_debug_tc_table(fft_size, sfmt, hop_bytes, 1.0, n_channels, None, digits, _ptr(plan), None, 0, None, None)
+    return dict(zip(TC_PLAN_FIELDS, (int(x) for x in plan)))
 
 
 def tc_table(fft_size: int, sfmt: int, hop_bytes: int, bins: Sequence[int], digits: int = 4, fullscale: float = 1.0):
     """Host-only view of the tensor-core K1's plan and coefficient table (abg_debug_tc_table).  Returns (plan dict,
     tab int8[K/32, 2, NC, 16], sq int64[C2p], cscale) or (plan, None, None, None) when the shape is not eligible."""
     L = load()
-    plan = np.zeros(13, np.int32)
     b = np.asarray(bins, np.int32)
-    L.abg_debug_tc_table(fft_size, sfmt, hop_bytes, fullscale, len(b), _ptr(b), digits, _ptr(plan), None, 0, None, None)
-    pd = dict(zip(TC_PLAN_FIELDS, (int(x) for x in plan)))
+    pd = tc_plan(fft_size, sfmt, hop_bytes, len(b), digits)
     if not pd["eligible"]:
         return pd, None, None, None
+    plan = np.zeros(len(TC_PLAN_FIELDS), np.int32)
     tab = np.zeros(pd["K"] * pd["NC"], np.int8)
     sq = np.zeros(pd["C2p"], np.int64)
     cs = C.c_double(0.0)
