@@ -354,10 +354,12 @@ ABG_API int abg_debug_run_outputs(abg_engine* e, int32_t* dims, float* wout, uns
  * writes these rows, so closed-squelch stretches are visible here.  Waits for the run; either pointer may be NULL. */
 ABG_API int abg_debug_k1_outputs(abg_engine* e, int32_t* dims, float* win, float* iqin);
 /* Feed |X[bin]| values straight into the demodulation state machine of one device (K1 skipped): wavein[C][n_batches *
- * WAVE_BATCH] becomes channel_t.wavein[AGC_EXTRA ...]; results are fetched as usual.  For the ports of the reference's own
- * Squelch / CTCSS unit tests (reference src/test_squelch.cpp:51-281, src/test_ctcss.cpp:122-155).  The device must not be
- * fed with abg_push and its channels must not need raw I/Q or AFC.  Returns the number of batches enqueued. */
-ABG_API int abg_debug_inject_wavein(abg_engine* e, int dev, int n_batches, const float* wavein);
+ * WAVE_BATCH] becomes channel_t.wavein[AGC_EXTRA ...], and iq_in[C][n_batches * WAVE_BATCH][2] (may be NULL) the X[bin]
+ * values of the same frames (channel_t.iq_in, where K1 would have stored them); results are fetched as usual.  For the
+ * ports of the reference's own Squelch / CTCSS unit tests (reference src/test_squelch.cpp:51-281, src/test_ctcss.cpp:122-155)
+ * and the exact comparisons of the demodulation kernel with the CPU oracle.  The device must not be fed with abg_push; its
+ * channels must not use AFC, and with iq_in == NULL must not need raw I/Q.  Returns the number of batches enqueued. */
+ABG_API int abg_debug_inject_wavein(abg_engine* e, int dev, int n_batches, const float* wavein, const float* iq_in);
 /* Measurement aid: per-role clock64 stamps of the tensor-core K1 (environment variable ABG_K1_TC_TRACE set at launch time);
  * out[256 CTAs][4 roles: producer, epilogue, loader, MMA][16 tiles][4 events]. */
 ABG_API int abg_debug_k1tc_trace(long long* out);

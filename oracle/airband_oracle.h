@@ -93,8 +93,9 @@ int abo_scan_select(void* h, int dev, int chan, int freq_idx);
 /* the stage boundaries, for tests: window[N]; one frame converted+windowed (2N floats) and its spectrum (2N) */
 int abo_get_window(void* h, float* window);
 int abo_debug_frame(void* h, int dev, const void* iq_frame, float* fftin, float* fftout);
-/* |X[bin]| values straight into the per-sample channel loop (K1 / FFT skipped): wavein[C][n_batches * WAVE_BATCH] */
-int abo_debug_inject_wavein(void* h, int dev, int n_batches, const float* wavein);
+/* |X[bin]| values straight into the per-sample channel loop (K1 / FFT skipped): wavein[C][n_batches * WAVE_BATCH], and the
+ * X[bin] values of the same frames iq_in[C][n_batches * WAVE_BATCH][2] (may be NULL: then no channel may need raw I/Q) */
+int abo_debug_inject_wavein(void* h, int dev, int n_batches, const float* wavein, const float* iq_in);
 
 /* ---- host-side config formulas (reference src/config.cpp, src/util.cpp) ------------------------------- */
 int32_t abo_calc_bin(int32_t freq, int32_t centerfreq, int32_t sample_rate, int32_t fft_size); /* config.cpp:666-667 */

@@ -516,18 +516,22 @@ long abo_run(void* h, int max_batches, int n_threads) {
     return total;
 }
 
-// stage tap (mirrors abg_debug_inject_wavein): wavein[C][n_batches * B] becomes channel_t.wavein[AGC_EXTRA ...], batch by batch
-int abo_debug_inject_wavein(void* h, int dev, int n_batches, const float* wavein) {
+// stage tap (mirrors abg_debug_inject_wavein): wavein[C][n_batches * B] becomes channel_t.wavein[AGC_EXTRA ...] and iq_in
+// [C][n_batches * B][2] channel_t.iq_in[2 * AGC_EXTRA ...] (where run_device() stores frame waveend), batch by batch
+int abo_debug_inject_wavein(void* h, int dev, int n_batches, const float* wavein, const float* iq_in) {
     Oracle* o = (Oracle*)h;
     if (dev < 0 || dev >= o->ndev() || n_batches < 1 || !wavein) return -1;
     Device& d = o->D(dev);
     const int B = o->wave_batch;
     for (auto& cp : d.ch)
-        if (cp->needs_raw_iq || cp->afc) return -1;
+        if ((cp->needs_raw_iq && !iq_in) || cp->afc) return -1;
     if (d.waveend != 0 && d.waveend != AGC_EXTRA) return -1;  // mixing injection with real frames is not supported
     for (int b = 0; b < n_batches; b++) {
-        for (size_t c = 0; c < d.ch.size(); c++)
+        for (size_t c = 0; c < d.ch.size(); c++) {
             memcpy(d.ch[c]->wavein.data() + AGC_EXTRA, wavein + (c * (size_t)n_batches + b) * B, sizeof(float) * B);
+            if (iq_in && d.ch[c]->needs_raw_iq)
+                memcpy(d.ch[c]->iq_in.data() + 2 * AGC_EXTRA, iq_in + 2 * ((c * (size_t)n_batches + b) * B), sizeof(float) * 2 * B);
+        }
         d.waveend = B + AGC_EXTRA;
         demod_batch(*o, d, nullptr);
     }

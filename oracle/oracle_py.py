@@ -70,7 +70,7 @@ def lib(variant: str = "restated"):
         "abo_scan_select": (i, [vp, i, i, i]),
         "abo_get_window": (i, [vp, vp]),
         "abo_debug_frame": (i, [vp, i, vp, vp, vp]),
-        "abo_debug_inject_wavein": (i, [vp, i, i, vp]),
+        "abo_debug_inject_wavein": (i, [vp, i, i, vp, vp]),
         "abo_calc_bin": (i32, [i32, i32, i32, i32]),
         "abo_calc_dm_dphi": (u32, [i32, i32, i32, i32]),
         "abo_dbfs_to_level": (f, [f, i32]),
@@ -206,11 +206,14 @@ class Oracle:
     def scan_select(self, dev: int, chan: int, freq_idx: int) -> None:
         assert self.L.abo_scan_select(self.h, dev, chan, freq_idx) == 0
 
-    def inject_wavein(self, dev: int, wavein: np.ndarray) -> int:
-        """Stage tap: wavein[C, n_batches * B] straight into the channel loop (FFT skipped)."""
+    def inject_wavein(self, dev: int, wavein: np.ndarray, iq: Optional[np.ndarray] = None) -> int:
+        """Stage tap: wavein[C, n_batches * B] straight into the channel loop (FFT skipped), with iq[C, n_batches * B]
+        (complex64) as the X[bin] values of the same frames for channels that need raw I/Q."""
         w = np.ascontiguousarray(wavein, np.float32)
         assert w.ndim == 2 and w.shape[1] % self.B == 0
-        return int(self.L.abo_debug_inject_wavein(self.h, dev, w.shape[1] // self.B, _ptr(w)))
+        q = None if iq is None else np.ascontiguousarray(iq, np.complex64)
+        assert q is None or q.shape == w.shape
+        return int(self.L.abo_debug_inject_wavein(self.h, dev, w.shape[1] // self.B, _ptr(w), _ptr(q)))
 
     def window(self) -> np.ndarray:
         w = np.empty(self.cfg.fft_size, np.float32)

@@ -1880,17 +1880,21 @@ int abg_debug_tc_table(int fft_size, int sfmt, int hop_bytes, float fullscale, i
     return ABG_OK;
 }
 
-// Stage tap for the upstream squelch / CTCSS behavioural tests (reference src/test_squelch.cpp, src/test_ctcss.cpp): feed
-// |X[bin]| values straight into the demodulation state machine.  wavein[C][n_batches * WAVE_BATCH] becomes
-// channel_t.wavein[AGC_EXTRA ...] of the device's channels (the AGC look-back keeps its initial 20.0, config.cpp:313-316, on
-// the first call and the previous tail afterwards), K1 is skipped, K2 runs n_batches batches, results are fetched as usual.
-// A device driven this way must not be fed with abg_push, and its channels must not need raw I/Q or AFC.
-int abg_debug_inject_wavein(abg_engine* e, int dev, int n_batches, const float* wavein) {
+// Stage tap for the upstream squelch / CTCSS behavioural tests (reference src/test_squelch.cpp, src/test_ctcss.cpp) and for
+// the exact K2-against-oracle tests: feed |X[bin]| values (and, optionally, X[bin] itself) straight into the demodulation
+// state machine.  wavein[C][n_batches * WAVE_BATCH] becomes channel_t.wavein[AGC_EXTRA ...] of the device's channels (the AGC
+// look-back keeps its initial 20.0, config.cpp:313-316, on the first call and the previous tail afterwards); iq_in[C][n_batches
+// * WAVE_BATCH][2], if given, goes to the iqin rows K1 would have filled for the same frames.  K1 is skipped, K2 runs n_batches
+// batches, results are fetched as usual.  A device driven this way must not be fed with abg_push; without iq_in its channels
+// must not need raw I/Q, and AFC channels are refused either way (AFC reads the spectrum of the batch's last frame).
+int abg_debug_inject_wavein(abg_engine* e, int dev, int n_batches, const float* wavein, const float* iq_in) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_debug_inject_wavein: device %d out of range", dev);
     if (n_batches < 1 || n_batches > e->nbmax || !wavein) return fail(ABG_EINVAL, "abg_debug_inject_wavein: n_batches must be 1..%d", e->nbmax);
     Device& d = e->dev[dev];
-    for (int c = 0; c < d.C; c++)
-        if (e->h_params[d.g0 + c].needs_raw_iq || e->h_params[d.g0 + c].afc) return fail(ABG_EINVAL, "abg_debug_inject_wavein: channel %d needs raw I/Q or AFC", c);
+    for (int c = 0; c < d.C; c++) {
+        if (e->h_params[d.g0 + c].afc) return fail(ABG_EINVAL, "abg_debug_inject_wavein: channel %d uses AFC", c);
+        if (e->h_params[d.g0 + c].needs_raw_iq && !iq_in) return fail(ABG_EINVAL, "abg_debug_inject_wavein: channel %d needs raw I/Q (iq_in)", c);
+    }
     cudaSetDevice(e->cuda_dev);
     CU(cudaStreamSynchronize(e->stream_c));
     CU(cudaStreamSynchronize(e->stream));
@@ -1902,6 +1906,13 @@ int abg_debug_inject_wavein(abg_engine* e, int dev, int n_batches, const float* 
         for (size_t r = 0; r < rows; r++) tm[r * d.C + c] = wavein[(size_t)c * rows + r];
     CU(cudaMemcpy2D(e->win[cur].p + (size_t)ABG_AGC_EXTRA * e->Gp + d.g0, sizeof(float) * e->Gp, tm.data(), sizeof(float) * d.C, sizeof(float) * d.C, rows,
                     cudaMemcpyHostToDevice));
+    if (iq_in) {
+        std::vector<float2> tq(rows * d.C);
+        for (int c = 0; c < d.C; c++)
+            for (size_t r = 0; r < rows; r++) tq[r * d.C + c] = make_float2(iq_in[2 * ((size_t)c * rows + r)], iq_in[2 * ((size_t)c * rows + r) + 1]);
+        CU(cudaMemcpy2D(e->iqin[cur].p + (size_t)ABG_AGC_EXTRA * e->Gp + d.g0, sizeof(float2) * e->Gp, tq.data(), sizeof(float2) * d.C, sizeof(float2) * d.C,
+                        rows, cudaMemcpyHostToDevice));
+    }
     std::vector<int> nb(e->dev.size(), 0);
     nb[dev] = n_batches;
     int n = 0;

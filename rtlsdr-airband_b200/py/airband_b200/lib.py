@@ -109,7 +109,7 @@ def load():
     L.abg_scan_select.restype, L.abg_scan_select.argtypes = i, [vp, i, i, i]
     L.abg_debug_timeline.restype, L.abg_debug_timeline.argtypes = i, [vp, i, C.POINTER(C.c_float)]
     L.abg_fft_path.restype, L.abg_fft_path.argtypes = i, [vp, i]
-    L.abg_debug_inject_wavein.restype, L.abg_debug_inject_wavein.argtypes = i, [vp, i, i, vp]
+    L.abg_debug_inject_wavein.restype, L.abg_debug_inject_wavein.argtypes = i, [vp, i, i, vp, vp]
     L.abg_debug_k1tc_trace.restype, L.abg_debug_k1tc_trace.argtypes = i, [vp]
     L.abg_debug_k2_stats.restype, L.abg_debug_k2_stats.argtypes = i, [vp]
     L.abg_spectrum_configure.restype, L.abg_spectrum_configure.argtypes = i, [vp, i, i]
@@ -383,11 +383,14 @@ class Engine:
         self._chk(self.L.abg_mixer_device_buffers(self.h, C.byref(a), C.byref(b)))
         return a.value, b.value
 
-    def inject_wavein(self, dev: int, wavein: np.ndarray) -> int:
-        """Stage tap: wavein[C, n_batches * B] straight into the demodulation state machine (K1 skipped)."""
+    def inject_wavein(self, dev: int, wavein: np.ndarray, iq: Optional[np.ndarray] = None) -> int:
+        """Stage tap: wavein[C, n_batches * B] straight into the demodulation state machine (K1 skipped), with iq[C,
+        n_batches * B] (complex64) as the X[bin] values of the same frames for channels that need raw I/Q."""
         w = np.ascontiguousarray(wavein, np.float32)
         assert w.ndim == 2 and w.shape[1] % self.B == 0
-        return self._chk(self.L.abg_debug_inject_wavein(self.h, dev, w.shape[1] // self.B, _ptr(w)))
+        q = None if iq is None else np.ascontiguousarray(iq, np.complex64)
+        assert q is None or q.shape == w.shape
+        return self._chk(self.L.abg_debug_inject_wavein(self.h, dev, w.shape[1] // self.B, _ptr(w), _ptr(q)))
 
     # ---- stage tap ------------------------------------------------------------------------------------------------
     def debug_frame(self, dev: int, raw_frame: np.ndarray) -> np.ndarray:

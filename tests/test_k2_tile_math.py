@@ -179,3 +179,163 @@ def test_am_agc_recurrence_without_the_clip_inside_a_committed_tile():
             calm = calm and abs(F(lag[k] - a_tile)) < F(a_tile * F(1.199985))
         if calm:
             assert not clipped and bits(a_seq) == bits(a_tile)
+
+
+# ---- the guard bands and range tests of k2_demod.cu, read from the source so that the checks below test the kernel's own
+# constants.  The reference decides the AM clip from the rounded quotient, |fl(n / d)| > 0.8f with d = fl(1.5 agc)
+# (rtl_airband.cpp:556-562); the kernel decides it without the division wherever |n| is far enough from 0.8 d, and falls
+# back (refuses the tile / block, or divides exactly) elsewhere.  A "decided" outcome must therefore equal the reference's.
+import os
+import re
+
+K2_SRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "rtlsdr-airband_b200", "csrc", "k2_demod.cu")
+
+
+def _k2_source():
+    with open(K2_SRC) as f:
+        return f.read()
+
+
+def _body(src, start):
+    """Source from `start` to the end of that definition (a function body or a macro)."""
+    i = src.index(start)
+    j = src.find("\n}\n", i)
+    k = src.find("#undef", i)
+    return src[i:min(x for x in (j, k) if x > 0)]
+
+
+def _hexf(s):
+    return float.fromhex(s.rstrip("f"))
+
+
+def _band_constants():
+    src = _k2_source()
+    run = _body(src, "__device__ __forceinline__ bool k2_open_run(")
+    tile = _body(src, "__device__ __forceinline__ bool k2_am_tile(")
+    samp = _body(src, "#define K2_OPEN_SAMPLE(")
+    c = {
+        "run_hi": re.search(r"an > a2 \* ([0-9.]+)f", run).group(1),
+        "run_lo": re.search(r"an < a2 \* ([0-9.]+)f", run).group(1),
+        "tile_lo": re.search(r"calm = an < a2k \* ([0-9.]+)f", tile).group(1),
+        "samp_hi": re.search(r"an > dd \* ([0-9.]+)f", samp).group(1),
+        "samp_lo": re.search(r"an < dd \* ([0-9.]+)f", samp).group(1),
+    }
+    rng = {}
+    for name, body, d in (("run", run, "d_"), ("tile", tile, "d_"), ("samp", samp, "dd")):
+        m = re.search(r"%s >= (0x1p-?\d+)f && %s <= (0x1p-?\d+)f && an >= (0x1p-?\d+)f && an <= (0x1p-?\d+)f" % (d, d), body)
+        rng[name] = tuple(_hexf(x) for x in m.groups())
+    return {k: F(float(v)) for k, v in c.items()}, rng
+
+
+def _operands(rng, n):
+    """(an, a2): agc values over the whole positive float32 range (subnormals included); |numerator| mostly within +-4e-5
+    (relative) of 1.2 agc = 0.8 * 1.5 agc, where the guard bands sit, some ulp steps either side of 0.8 * fl(1.5 agc), and
+    some anywhere."""
+    e = rng.integers(0, 255, n, dtype=np.uint32)
+    m = rng.integers(0, 1 << 23, n, dtype=np.uint32)
+    a2 = ((e << 23) | m).view(np.float32)
+    with np.errstate(over="ignore", under="ignore", invalid="ignore"):
+        d = (a2 * F(1.5)).astype(F)
+        kind = rng.integers(0, 8, n)
+        rel = np.where(kind < 5, rng.uniform(-4e-5, 4e-5, n), rng.uniform(-1.6e-5, -1.4e-5, n) * rng.choice([-1, 1], n))
+        an = (a2.astype(np.float64) * 1.2 * (1.0 + rel)).astype(F)
+        steps = rng.integers(-64, 65, n)
+        near = (d.astype(np.float64) * np.float64(F(0.8))).astype(F)
+        near = (near.view(np.int32) + steps.astype(np.int32)).view(np.float32)
+        an = np.where(kind == 6, np.abs(near), an)
+        wild = ((rng.integers(0, 255, n, dtype=np.uint32) << 23) | rng.integers(0, 1 << 23, n, dtype=np.uint32)).view(np.float32)
+        an = np.where(kind == 7, wild, an)
+    ok = np.isfinite(an) & np.isfinite(a2) & (a2 > 0)
+    return an[ok].astype(F), a2[ok].astype(F)
+
+
+def test_agc_clip_guard_bands_decide_like_the_rounded_quotient():
+    """About 10^7 operand pairs through the three division-free forms of the |n / d| > 0.8f decision: k2_open_run (big /
+    not big outside a band around 1.2 agc), k2_am_tile (`calm`: certainly not big) and K2_OPEN_SAMPLE (big / not big outside a
+    band around 0.8 d).  Wherever a form counts as decided, its answer equals |fl(n / d)| > 0.8f."""
+    c, rngs = _band_constants()
+    rng = np.random.default_rng(62)
+    inside = {"run": 0, "tile": 0, "samp": 0}
+    decided = {"run": 0, "tile": 0, "samp": 0}
+    total = 0
+    for _ in range(10):
+        an, a2 = _operands(rng, 1_000_000)
+        total += an.size
+        with np.errstate(over="ignore", under="ignore", invalid="ignore", divide="ignore"):
+            d = (a2 * F(1.5)).astype(F)
+            q = (an / d).astype(F)
+            truth = np.abs(q) > F(0.8)
+            inside_band = np.abs(an.astype(np.float64) / (1.2 * a2.astype(np.float64)) - 1.0) < 1e-5
+
+            def in_range(name):
+                dl, dh, nl, nh = rngs[name]
+                return (d >= F(dl)) & (d <= F(dh)) & (an >= F(nl)) & (an <= F(nh))
+            big = an > (a2 * c["run_hi"]).astype(F)
+            ok = (big | (an < (a2 * c["run_lo"]).astype(F))) & in_range("run")
+            assert np.array_equal(big[ok], truth[ok]), "k2_open_run decides the clip wrongly"
+            decided["run"] += int(ok.sum()); inside["run"] += int((ok & inside_band).sum())
+            calm = (an < (a2 * c["tile_lo"]).astype(F)) & in_range("tile")
+            assert not truth[calm].any(), "k2_am_tile commits a tile in which a sample clips"
+            decided["tile"] += int(calm.sum()); inside["tile"] += int((calm & inside_band).sum())
+            bigs = an > (d * c["samp_hi"]).astype(F)
+            sure = (bigs | (an < (d * c["samp_lo"]).astype(F))) & in_range("samp")
+            assert np.array_equal(bigs[sure], truth[sure]), "K2_OPEN_SAMPLE decides the clip wrongly"
+            decided["samp"] += int(sure.sum()); inside["samp"] += int((sure & inside_band).sum())
+    assert total > 9_000_000
+    # the operands really straddle the bands: most pairs are decided, and the undecided ones are the ones near 1.2 agc
+    for k in decided:
+        assert 0.1 * total < decided[k] < total, (k, decided[k], total)
+        assert inside[k] == 0, (k, inside[k])
+
+
+def _range_predicates():
+    src = _k2_source()
+    sq = re.search(r"bool k2_sqrt_ordinary_ok\(float x\) \{ return x >= (0x1p-?\d+)f && x <= (0x1p-?\d+)f; \}", src)
+    dv = re.search(r"return ad >= (0x1p-?\d+)f && ad <= (0x1p-?\d+)f && an <= (0x1p-?\d+)f && \(an >= (0x1p-?\d+)f \|\| an == 0\.0f\);", src)
+    assert sq and dv, "k2_sqrt_ordinary_ok / k2_div_ok changed shape: update this test"
+    slo, shi = (F(_hexf(x)) for x in sq.groups())
+    dlo, dhi, nhi, nlo = (F(_hexf(x)) for x in dv.groups())
+
+    def sqrt_ok(x):
+        return (x >= slo) & (x <= shi)
+
+    def div_ok(n, d):
+        an, ad = np.abs(n), np.abs(d)
+        return (ad >= dlo) & (ad <= dhi) & (an <= nhi) & ((an >= nlo) | (an == F(0.0)))
+    return sqrt_ok, div_ok
+
+
+def _every_exponent():
+    """Both signs, every exponent field (subnormals and inf / NaN included), mantissas 0, 1, a middle one and all ones."""
+    e = np.arange(256, dtype=np.uint32)
+    m = np.array([0, 1, 0x2aaaab, 0x7fffff], np.uint32)
+    u = ((e[:, None] << 23) | m[None, :]).ravel()
+    return np.concatenate([u, u | np.uint32(0x80000000)]).view(np.float32)
+
+
+def test_sqrt_and_division_range_tests_admit_nothing_outside_the_documented_ranges():
+    """k2_sqrt_ordinary (rsqrt.approx + one correction) equals sqrt.rn only on [2^-100, 2^125]; k2_div_ordinary (rcp.approx +
+    Newton + remainder correction) equals div.rn only for |d| in [2^-62, 2^62] and |n| in [2^-62, 2^62] or n == 0.  The range
+    tests must admit nothing outside, and everything inside."""
+    sqrt_ok, div_ok = _range_predicates()
+    x = _every_exponent()
+    with np.errstate(invalid="ignore"):
+        inside = (x >= F(2.0 ** -100)) & (x <= F(2.0 ** 125))
+        got = sqrt_ok(x)
+    assert not (got & ~inside).any(), x[got & ~inside][:8]
+    assert got[inside].all()
+    # the boundaries themselves and their neighbours
+    for b in (2.0 ** -100, 2.0 ** 125):
+        b = F(b)
+        lo, hi = np.nextafter(b, F(0)), np.nextafter(b, F(np.inf))
+        assert sqrt_ok(np.array([b]))[0]
+        assert not sqrt_ok(np.array([lo if b < 1 else hi]))[0]
+    n = np.repeat(x, x.size)
+    d = np.tile(x, x.size)
+    with np.errstate(invalid="ignore"):
+        an, ad = np.abs(n), np.abs(d)
+        r = F(2.0 ** 62)
+        ok_doc = (ad >= F(1) / r) & (ad <= r) & (((an >= F(1) / r) & (an <= r)) | (an == 0))
+        got = div_ok(n, d)
+    assert not (got & ~ok_doc).any(), (n[got & ~ok_doc][:4], d[got & ~ok_doc][:4])
+    assert got[ok_doc].all()

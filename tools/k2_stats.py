@@ -17,7 +17,12 @@ NAMES = {0: "samples", 1: "general-path samples", 2: "tile attempts OPEN", 3: "t
          12: "no room for a tile", 13: "CTCSS window ends in tile", 14: "post estimator not live", 15: "OPENING at buffer_size boundary", 16: "CLOSED recent_open pending",
          17: "tiles of 8", 18: "tiles of 16", 20: "  .. state ends within 8", 22: "tile attempts held-CLOSED", 23: "tile samples held-CLOSED", 31: "refused: held-CLOSED ends", 21: "  .. noise-floor update within 8", 24: "refused: low_signal_abort", 25: "refused: lp division range",
          26: "refused: sqrt range", 27: "refused: has_signal false", 28: "refused: CLOSED sees signal", 29: "refused: post < tail", 30: "refused: discriminator division range",
-         32: "general in CLOSED", 33: "general in OPENING", 34: "general in CLOSING", 35: "general in ABORT", 36: "general in OPEN", 40: "general: transition sample"}
+         32: "general in CLOSED", 33: "general in OPENING", 34: "general in CLOSING", 35: "general in ABORT", 36: "general in OPEN", 40: "general: transition sample",
+         41: "AM tile attempts OPEN", 42: "AM tile samples OPEN", 43: "AM tile refused OPEN", 44: "AM tile attempts quiet", 45: "AM tile samples quiet",
+         46: "AM tile refused quiet", 47: "AM OPEN tile fully capped", 48: "AM OPEN tile never capped", 57: "AM quiet tile never capped",
+         49: "AM open_run attempts (LPW>=2)", 50: "AM open_run refused", 51: "AM quiet_run attempts (LPW>=2)", 52: "AM quiet_run refused",
+         53: "AM open sample: exact division", 54: "NFM block attempts OPEN/CLOSING (LPW 2)", 55: "NFM block attempts OPENING", 56: "NFM block attempts CLOSED",
+         58: "NFM block samples", 59: "NFM block refused"}
 
 
 def main():
