@@ -320,6 +320,47 @@ ABG_API int abg_fetch_input_levels(abg_engine* e, int dev, abg_input_levels* out
  * (0 if that run metered nothing).  Waits for it. */
 ABG_API int abg_debug_input_meter_time(abg_engine* e, float* ms);
 
+/* Sub-band I/Q outputs (not part of the reference surface: a channel's iq_out is one FFT bin at WAVE_RATE and zero while
+ * its squelch is closed, so a decoder of a wider or ungated signal, or a recorder of a whole sub-band, would otherwise
+ * need a dongle of its own).  Each device has up to ABG_SUBBAND_MAX outputs; output k of device dev is a digital
+ * down-converter: mixer, FIR low-pass and decimator, computed on the GPU from the raw samples the engine already holds.
+ * With offset_hz, decimation D (1 <= D <= WAVE_BATCH * hop) and real coefficients h[0..L) (1 <= L <= ABG_SUBBAND_MAX_COEFFS):
+ *     v[s]  = complex level of absolute sample s (counted from the device's first pushed sample), the input meter's
+ *             float32 conversion: U8 (c - 127.5f) / 127.5f, S8 c / 128.0f, S16 / F32 (1.0f / fullscale) * x
+ *     delta = llround(offset_hz / sample_rate * 2^32) mod 2^32; the output's true frequency is delta * sample_rate / 2^32
+ *             folded into [-sample_rate/2, sample_rate/2)
+ *     y[m]  = sum_{j=0}^{L-1} h[j] * v[mD - j] * exp(-2 pi i ((delta * (mD - j)) mod 2^32) / 2^32)
+ * The phase is exact integer arithmetic on the absolute sample index: the oscillator neither drifts nor depends on how
+ * batches are grouped.  Batch b (numbered as for the band spectrum) covers the input meter's samples s in [s0, s0 + n),
+ * s0 = (AGC_EXTRA + b*WAVE_BATCH) * hop, n = WAVE_BATCH * hop, and carries the outputs m with s0 <= mD < s0 + n:
+ * m = ceil(s0 / D) .. ceil((s0 + n) / D) - 1, floor(n / D) or ceil(n / D) of them.  An output's input starts at s0 of the
+ * first batch it covers after it was switched on or reconfigured; earlier samples count as zero, so its first L - 1
+ * outputs carry the filter's start-up transient.  A scan-mode retune moves the centre frequency and the output with it.
+ * Each y[m] is summed in a fixed order that depends on (m, L) only: outputs are bitwise reproducible for every
+ * max_batches_per_run, push pattern and fft_mode.  Against float64 each output is within a few L * 2^-24 * sum|h| * max|v|.
+ * Computed by one extra kernel per run on the K1 stream, after K1 and the other monitors; K2 does not wait for it.  While
+ * any output of a device is on, abg_push's compaction keeps (L_max - 1) samples before the next unconsumed one (L_max:
+ * the longest filter switched on), so the input buffer holds up to that many samples less of new input than
+ * input_capacity_batches says.  With every output off (the default) nothing is launched, allocated or copied and
+ * compaction is unchanged.  Resident runs (abg_run_resident) compute outputs over the resident buffer (samples before it
+ * count as zero) but queue none; batches fed through abg_debug_inject_wavein have no samples and produce none. */
+#define ABG_SUBBAND_MAX 8
+#define ABG_SUBBAND_MAX_COEFFS 4096
+/* abg_subband_configure: decim = 0 switches output k off; otherwise it is (re)configured and restarts, for batches
+ * enqueued by later abg_run / abg_run_resident calls.  ABG_ERANGE for a bad dev or k; ABG_EINVAL for |offset_hz| >
+ * sample_rate / 2 (or not finite), decim outside [0, WAVE_BATCH * hop], n_coeffs outside [1, ABG_SUBBAND_MAX_COEFFS],
+ * null coeffs or a coefficient that is not finite.  Waits for the engine's K1 stream. */
+ABG_API int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int decim, int n_coeffs, const float* coeffs);
+/* Pop the oldest unfetched batch of output k: iq[2 * n_samples] interleaved cf32 (room for 2 * ceil(n / D) floats; may be
+ * NULL), batch_seq as for abg_fetch_spectrum, first_index = m of its first output (gaps show in both), n_samples.
+ * Returns 1 if one was popped, 0 if none is ready, < 0 on error; waits for the run that computed it.  Lossy like the
+ * spectrum's queue: max_batches_per_run + 2 batches per output, the oldest overwritten first; never holds a result slot or
+ * causes ABG_EOVERFLOW, and batches already queued stay fetchable after the output is switched off or reconfigured. */
+ABG_API int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t* batch_seq, uint64_t* first_index, int32_t* n_samples);
+/* Measurement aid: device time of the sub-band kernel of the most recent run, from CUDA events around it on the K1 stream
+ * (0 if that run computed no output).  Waits for it. */
+ABG_API int abg_debug_subband_time(abg_engine* e, float* ms);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

@@ -15,6 +15,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/airband_b200.h"
+
 #include <mutex>
 
 // Kernel function attributes (dynamic shared-memory opt-in, carveout) are per CUDA device: several engines may live on
@@ -225,6 +227,34 @@ struct InmArgs {
 };
 cudaError_t abg_launch_input_meter(const InmArgs& a, int n_devices, int max_items, cudaStream_t s);
 int abg_input_meter_chunks(int batch_bytes);  // work items per batch of a device
+
+// sub-band I/Q outputs (subband.cu): see abg_subband_configure in include/airband_b200.h
+struct SbOut {  // one switched-on output
+    const float2* coef;      // [n_coeffs] h[j] * exp(+2 pi i delta j / 2^32), built in double, stored as float32
+    unsigned char* ring;     // device view of the page-locked result ring [ring_cap][entry_bytes]
+    uint32_t delta;          // phase step per sample, 2^-32 turns
+    int32_t decim, n_coeffs, ring_cap, entry_bytes;
+};
+struct SbCfg {  // per device with an output on; written by abg_subband_configure
+    SbOut out[ABG_SUBBAND_MAX];
+    int32_t n_out, sfmt, bpc, batch_samples, n_chunks;
+    int32_t hist;            // L_max - 1: history samples staged before each chunk
+    float scale;             // 1.0f / fullscale (S16, F32)
+};
+struct SbRun {  // per device with an output on; uploaded with every run
+    const unsigned char* raw;
+    long long base;          // absolute sample index of raw[0]; samples below it read as zero
+    long long s0;            // absolute sample index of the run's first batch
+    int32_t n_batches;       // batches of this run (0 = none)
+    int32_t ring_pos0[ABG_SUBBAND_MAX];  // ring entry of the run's first batch per output; < 0: resident run, no output
+    int32_t lead[ABG_SUBBAND_MAX];       // s0 - (first input sample of the output), at most 2^30: earlier samples are zero
+};
+struct SbArgs {
+    const SbCfg* cfg;  // [devices with an output on]
+    const SbRun* run;
+};
+cudaError_t abg_launch_subband(const SbArgs& a, int n_devices, int max_items, int max_hist, cudaStream_t s);
+int abg_subband_chunks(int batch_samples);  // work items per batch of a device
 
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B

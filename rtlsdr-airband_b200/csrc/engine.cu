@@ -18,6 +18,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <complex>
 #include <deque>
 #include <memory>
@@ -197,6 +198,21 @@ struct MonitorQueue {
         if (ring) cudaFreeHost(ring);
         ring = nullptr;
     }
+    // Like alloc, for a monitor whose entry size can grow (sub-band outputs): a larger entry moves the ring, entry by
+    // entry, so that what is queued survives.  false: out of page-locked memory, the old ring is kept.
+    bool reserve(int cap_, size_t entry_bytes_) {
+        if (ring && entry_bytes_ <= entry_bytes) return true;
+        unsigned char* grown = nullptr;
+        if (cudaHostAlloc((void**)&grown, (size_t)cap_ * entry_bytes_, cudaHostAllocMapped) != cudaSuccess) return false;
+        if (ring) {
+            for (int i = 0; i < cap; i++) memcpy(grown + (size_t)i * entry_bytes_, ring + (size_t)i * entry_bytes, entry_bytes);
+            cudaFreeHost(ring);
+        }
+        ring = grown;
+        cap = cap_;
+        entry_bytes = entry_bytes_;
+        return true;
+    }
     // Queue the n batches of run `run` whose first is batch number seq0; returns the ring entry of the first.
     int queue(int n, uint64_t seq0, uint64_t run, int32_t n_frames) {
         const int pos0 = next;
@@ -236,6 +252,18 @@ struct Device {
     int inm_chunks = 0;
     void* inm_work = nullptr;    // device: histograms uint32[nbmax][2][256], counters int32[nbmax], chunk sums int64[nbmax][inm_chunks][ABG_INM_PARTIAL]; kept once allocated
     MonitorQueue inm_q;          // abg_input_levels per entry
+    // sub-band I/Q outputs (abg_subband_configure); nothing is allocated until one is first switched on
+    struct Subband {
+        bool on = false;
+        bool restart = false;        // the next streamed run starts the output's input at its first batch
+        int decim = 0, n_coeffs = 0, coef_cap = 0;
+        uint32_t delta = 0;
+        long long start = 0;         // absolute sample index of the output's first input sample
+        float2* coef = nullptr;      // device [coef_cap]: h[j] * exp(+2 pi i delta j / 2^32); kept once allocated
+        MonitorQueue q;              // cf32 [ceil(n / decim)] per entry, Entry.n_frames = decim
+    } sb[ABG_SUBBAND_MAX];
+    int sb_hist = 0;                 // L_max - 1 over the outputs switched on: samples compaction keeps before `consumed`
+    size_t dropped = 0;              // stream bytes compaction has dropped: raw[cur][0] is byte `dropped` of the stream
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -377,7 +405,8 @@ struct abg_engine {
     DevBuf<SpecRun> spec_run;                // room for every device
     std::vector<SpecRun> h_spec_run;
     cudaEvent_t ev_raw[2] = {nullptr, nullptr};   // after the last kernel that read raw[] (K1 aside: the band spectrum, the
-                                                  // input meter) of the latest run of each parity that ran one
+                                                  // input meter, the sub-band outputs) of the latest run of each parity
+                                                  // that ran one
     cudaEvent_t tl_spec[TL_RUNS][2] = {};    // spectrum kernel start / end of the last TL_RUNS runs
     bool spec_ran[TL_RUNS] = {};
     // carrier frequency meter
@@ -394,6 +423,14 @@ struct abg_engine {
     std::vector<InmRun> h_inm_run;
     cudaEvent_t tl_inm[TL_RUNS][2] = {};     // meter kernel start / end of the last TL_RUNS runs
     bool inm_ran[TL_RUNS] = {};
+    // sub-band I/Q outputs
+    std::vector<int> sb_devs;                // devices with an output on, in launch order (grid.y of the kernel)
+    DevBuf<SbCfg> sb_cfg;                    // [sb_devs.size()]
+    DevBuf<SbRun> sb_run;                    // room for every device
+    std::vector<SbRun> h_sb_run;
+    int sb_max_hist = 0;                     // largest Device::sb_hist of sb_devs
+    cudaEvent_t tl_sb[TL_RUNS][2] = {};      // sub-band kernel start / end of the last TL_RUNS runs
+    bool sb_ran[TL_RUNS] = {};
     // mixers (reference src/mixer.cpp)
     int n_mixers = 0;
     DevBuf<int32_t> mix_offsets;
@@ -433,10 +470,15 @@ void engine_free(abg_engine* e) {
         d.spec_q.release();
         d.car_q.release();
         d.inm_q.release();
+        for (auto& so : d.sb) {
+            if (so.coef) cudaFree(so.coef);
+            so.q.release();
+        }
     }
     e->spec_cfg.free(); e->spec_run.free();
     e->car_cfg.free(); e->car_run.free();
     e->inm_cfg.free(); e->inm_run.free();
+    e->sb_cfg.free(); e->sb_run.free();
     for (auto& row : e->tl_spec)
         for (auto& ev : row)
             if (ev) cudaEventDestroy(ev);
@@ -444,6 +486,9 @@ void engine_free(abg_engine* e) {
         for (auto& ev : row)
             if (ev) cudaEventDestroy(ev);
     for (auto& row : e->tl_inm)
+        for (auto& ev : row)
+            if (ev) cudaEventDestroy(ev);
+    for (auto& row : e->tl_sb)
         for (auto& ev : row)
             if (ev) cudaEventDestroy(ev);
     for (auto& g : e->groups) {
@@ -1059,6 +1104,52 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             e->inm_ran[ri % abg_engine::TL_RUNS] = true;
         }
     }
+    // ---- sub-band outputs of the devices with one on (stream A: after K1 and the monitors; reads raw[], so abg_push's
+    // compaction waits for it through ev_raw) ----
+    e->sb_ran[ri % abg_engine::TL_RUNS] = false;
+    if (!skip_k1 && !e->sb_devs.empty()) {
+        int max_items = 0;
+        for (size_t m = 0; m < e->sb_devs.size(); m++) {
+            Device& d = e->dev[e->sb_devs[m]];
+            const int n = nb[e->sb_devs[m]];
+            SbRun& r = e->h_sb_run[m];
+            const bool primed = resident ? d.res_primed : d.primed;
+            r.raw = resident ? d.res : d.raw[d.cur];
+            // the input meter's first byte of the run's first batch; a resident buffer is a stream of its own
+            const unsigned long long first_byte = resident ? (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes
+                                                           : (unsigned long long)d.consumed + (primed ? 0ull : (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes);
+            r.base = resident ? 0 : (long long)(d.dropped / d.bpc);
+            r.s0 = r.base + (long long)(first_byte / d.bpc);
+            r.n_batches = n;
+            int o = 0;
+            for (auto& so : d.sb) {
+                if (!so.on) continue;
+                if (!resident && n > 0 && so.restart) {
+                    so.start = r.s0;
+                    so.restart = false;
+                }
+                r.lead[o] = (int32_t)std::min<long long>(r.s0 - (resident ? 0 : so.start), 1ll << 30);
+                r.ring_pos0[o] = queue_outputs && n > 0 ? so.q.queue(n, d.batch_seq, ri, so.decim) : -1;
+                o++;
+            }
+            max_items = std::max(max_items, n * abg_subband_chunks(B * d.hop));
+        }
+        if (max_items > 0) {
+            const int nl = upload_small(e->sb_run.p, e->h_sb_run.data(), sizeof(SbRun) * e->sb_devs.size(), sa);
+            if (nl < 0) return fail(ABG_ECUDA, "sub-band parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+            e->launches += (uint64_t)nl;
+            SbArgs A{};
+            A.cfg = e->sb_cfg.p; A.run = e->sb_run.p;
+            cudaEvent_t* ts = e->tl_sb[ri % abg_engine::TL_RUNS];
+            CU(cudaEventRecord(ts[0], sa));
+            cudaError_t ers = abg_launch_subband(A, (int)e->sb_devs.size(), max_items, e->sb_max_hist, sa);
+            if (ers != cudaSuccess) return fail(ABG_ECUDA, "sub-band launch failed: %s", cudaGetErrorString(ers));
+            e->launches++;
+            CU(cudaEventRecord(ts[1], sa));
+            CU(cudaEventRecord(e->ev_raw[cur], sa));
+            e->sb_ran[ri % abg_engine::TL_RUNS] = true;
+        }
+    }
     // ---- K2 (stream B, after this run's K1; overlaps the next run's K1) ----
     CU(cudaStreamWaitEvent(sb, e->ev_k1[cur], 0));
     for (size_t i = 0; i < e->dev.size(); i++) {
@@ -1197,14 +1288,17 @@ int abg_push(abg_engine* e, int dev, const void* iq, size_t nbytes) {
     if (d.fill + nbytes > d.cap) {
         // compact: move the unconsumed tail to the front of the other buffer.  Ingest runs on its own stream so that
         // host->device copies overlap K1; the other buffer may still be read by the most recent K1, so wait for it.
-        const size_t keep_from = d.consumed & ~(size_t)15;  // keep the copy 16-byte aligned on both sides
+        // keep the copy 16-byte aligned on both sides; with a sub-band output on, keep its filter's history too
+        const size_t hist = (size_t)d.sb_hist * d.bpc;
+        const size_t keep_from = (d.consumed > hist ? d.consumed - hist : 0) & ~(size_t)15;
         const size_t rem = d.fill - keep_from;
         if (rem + nbytes > d.cap) {
             return fail(ABG_EOVERFLOW, "abg_push: device %d input buffer overflow (%zu buffered + %zu new > %zu)", dev, d.fill - d.consumed, nbytes, d.cap);
         }
         // the destination buffer was last read by a K1 launched before the previous compaction: with at least one run since
         // then that is run_index-2 or older, so the copy overlaps the K1 that is reading the current buffer right now
-        // (the band spectrum and the input meter read the same bytes right after that K1: ev_raw follows the last of them)
+        // (the band spectrum, the input meter and the sub-band outputs read the same bytes right after that K1: ev_raw
+        // follows the last of them)
         if (d.runs_since_compaction >= 1) {
             if (e->run_index >= 2) {
                 CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 2) & 1], 0));
@@ -1219,6 +1313,7 @@ int abg_push(abg_engine* e, int dev, const void* iq, size_t nbytes) {
         d.cur ^= 1;
         d.fill = rem;
         d.consumed -= keep_from;
+        d.dropped += keep_from;
     }
     CU(cudaMemcpyAsync(d.raw[d.cur] + d.fill, iq, nbytes, cudaMemcpyHostToDevice, e->stream_c));
     e->ingest_dirty = true;
@@ -1369,7 +1464,7 @@ int abg_fft_path(const abg_engine* e, int dev) {
     return g.use_tc ? 3 : (g.pruned ? 2 : 1);
 }
 
-// The monitors that read raw[] after K1 (band spectrum, input meter) record ev_raw, which abg_push's compaction waits for.
+// The monitors that read raw[] after K1 (band spectrum, input meter, sub-band outputs) record ev_raw, which abg_push's compaction waits for.
 static int create_raw_events(abg_engine* e) {
     if (e->ev_raw[0]) return ABG_OK;
     for (int k = 0; k < 2; k++) CU(cudaEventCreateWithFlags(&e->ev_raw[k], cudaEventDisableTiming));
@@ -1605,6 +1700,124 @@ int abg_debug_input_meter_time(abg_engine* e, float* ms) {
     if (e->run_index == 0 || !e->inm_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
     cudaSetDevice(e->cuda_dev);
     cudaEvent_t* ts = e->tl_inm[(e->run_index - 1) % abg_engine::TL_RUNS];
+    CU(cudaEventSynchronize(ts[1]));
+    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
+    return ABG_OK;
+}
+
+// ---- sub-band I/Q outputs (definition in airband_b200.h) ---------------------------------------------------------------
+int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int decim, int n_coeffs, const float* coeffs) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_subband_configure: device %d out of range", dev);
+    if (k < 0 || k >= ABG_SUBBAND_MAX) return fail(ABG_ERANGE, "abg_subband_configure: output %d out of range [0, %d)", k, ABG_SUBBAND_MAX);
+    Device& d = e->dev[dev];
+    const int n = e->B * d.hop;  // samples per batch
+    if (decim < 0 || decim > n) return fail(ABG_EINVAL, "abg_subband_configure: decimation %d outside [0, %d]", decim, n);
+    if (decim > 0) {
+        if (!std::isfinite(offset_hz) || fabs(offset_hz) > d.sample_rate / 2.0)
+            return fail(ABG_EINVAL, "abg_subband_configure: offset %g Hz outside +-sample_rate/2", offset_hz);
+        if (n_coeffs < 1 || n_coeffs > ABG_SUBBAND_MAX_COEFFS)
+            return fail(ABG_EINVAL, "abg_subband_configure: %d coefficients outside [1, %d]", n_coeffs, ABG_SUBBAND_MAX_COEFFS);
+        if (!coeffs) return fail(ABG_EINVAL, "abg_subband_configure: null coefficients");
+        for (int j = 0; j < n_coeffs; j++)
+            if (!std::isfinite(coeffs[j])) return fail(ABG_EINVAL, "abg_subband_configure: coefficient %d is not finite", j);
+    }
+    Device::Subband& so = d.sb[k];
+    if (decim == 0 && !so.on) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream));  // an enqueued kernel may still read the tables, the coefficients or the ring
+    if (decim > 0) {
+        if (!e->tl_sb[0][0])
+            for (auto& row : e->tl_sb)
+                for (auto& ev : row) CU(cudaEventCreate(&ev));
+        if (create_raw_events(e) != ABG_OK) return ABG_ECUDA;
+        // delta = llround(offset / fs * 2^32) mod 2^32; g[j] = h[j] exp(+2 pi i delta j / 2^32) in double, then float32
+        const uint32_t delta = (uint32_t)(unsigned long long)llround(offset_hz / d.sample_rate * 4294967296.0);
+        std::vector<float2> g(n_coeffs);
+        for (int j = 0; j < n_coeffs; j++) {
+            const double turns = (double)(int32_t)(delta * (uint32_t)j) * 0x1p-32;  // exact, in [-1/2, 1/2)
+            const double a = 2.0 * M_PI * turns;
+            g[j] = make_float2((float)(coeffs[j] * cos(a)), (float)(coeffs[j] * sin(a)));
+        }
+        if (so.coef_cap < n_coeffs) {
+            if (so.coef) cudaFree(so.coef);
+            so.coef = nullptr;
+            so.coef_cap = 0;
+            if (cudaMalloc((void**)&so.coef, sizeof(float2) * n_coeffs) != cudaSuccess) {
+                so.coef = nullptr;
+                return fail(ABG_ENOMEM, "Out of device memory for the sub-band coefficients of device %d", dev);
+            }
+            so.coef_cap = n_coeffs;
+        }
+        CU(cudaMemcpy(so.coef, g.data(), sizeof(float2) * n_coeffs, cudaMemcpyHostToDevice));
+        if (!so.q.reserve(e->nbmax + 2, sizeof(float2) * (size_t)((n + decim - 1) / decim)))
+            return fail(ABG_ENOMEM, "Out of page-locked host memory for the sub-band ring");
+        so.decim = decim;
+        so.n_coeffs = n_coeffs;
+        so.delta = delta;
+        so.restart = true;
+    }
+    so.on = decim > 0;
+    d.sb_hist = 0;
+    for (const auto& x : d.sb)
+        if (x.on) d.sb_hist = std::max(d.sb_hist, x.n_coeffs - 1);
+    // rebuild the launch's device list and its static table
+    e->sb_devs.clear();
+    e->sb_max_hist = 0;
+    std::vector<SbCfg> cfgs;
+    for (int i = 0; i < (int)e->dev.size(); i++) {
+        const Device& x = e->dev[i];
+        SbCfg c{};
+        for (const auto& y : x.sb) {
+            if (!y.on) continue;
+            SbOut& o = c.out[c.n_out++];
+            o.coef = y.coef;
+            CU(cudaHostGetDevicePointer((void**)&o.ring, y.q.ring, 0));
+            o.delta = y.delta; o.decim = y.decim; o.n_coeffs = y.n_coeffs;
+            o.ring_cap = y.q.cap; o.entry_bytes = (int32_t)y.q.entry_bytes;
+        }
+        if (c.n_out == 0) continue;
+        c.sfmt = x.sfmt; c.bpc = x.bpc; c.batch_samples = e->B * x.hop; c.n_chunks = abg_subband_chunks(c.batch_samples);
+        c.hist = x.sb_hist;
+        c.scale = 1.0f / x.fullscale;
+        e->sb_max_hist = std::max(e->sb_max_hist, x.sb_hist);
+        e->sb_devs.push_back(i);
+        cfgs.push_back(c);
+    }
+    e->sb_cfg.free();
+    e->h_sb_run.assign(e->sb_devs.size(), SbRun{});
+    if (cfgs.empty()) return ABG_OK;
+    if (e->sb_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the sub-band tables");
+    CU(cudaMemcpy(e->sb_cfg.p, cfgs.data(), sizeof(SbCfg) * cfgs.size(), cudaMemcpyHostToDevice));
+    // upload_small writes whole 16-byte words: room for every device plus the rounding
+    if (!e->sb_run.p && e->sb_run.alloc(e->dev.size() + 1)) return fail(ABG_ENOMEM, "Out of device memory for the sub-band tables");
+    return ABG_OK;
+}
+
+int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t* batch_seq, uint64_t* first_index, int32_t* n_samples) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_subband: device %d out of range", dev);
+    if (k < 0 || k >= ABG_SUBBAND_MAX) return fail(ABG_ERANGE, "abg_fetch_subband: output %d out of range [0, %d)", k, ABG_SUBBAND_MAX);
+    const Device& d = e->dev[dev];
+    const unsigned char* src = nullptr;
+    MonitorQueue::Entry r{};
+    const int rc = monitor_pop(e, e->dev[dev].sb[k].q, e->tl_sb, &src, &r);
+    if (rc <= 0) return rc;
+    // the batch's outputs: s0 <= mD < s0 + n with D the decimation the batch was computed with
+    const unsigned long long n = (unsigned long long)e->B * d.hop, D = (unsigned long long)r.n_frames;
+    const unsigned long long s0 = ((unsigned long long)ABG_AGC_EXTRA + r.seq * e->B) * d.hop;
+    const unsigned long long m0 = (s0 + D - 1) / D, m1 = (s0 + n + D - 1) / D;
+    if (iq) memcpy(iq, src, sizeof(float2) * (m1 - m0));
+    if (batch_seq) *batch_seq = r.seq;
+    if (first_index) *first_index = m0;
+    if (n_samples) *n_samples = (int32_t)(m1 - m0);
+    return 1;
+}
+
+int abg_debug_subband_time(abg_engine* e, float* ms) {
+    if (!ms) return fail(ABG_EINVAL, "abg_debug_subband_time: null argument");
+    *ms = 0.0f;
+    if (e->run_index == 0 || !e->sb_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    cudaEvent_t* ts = e->tl_sb[(e->run_index - 1) % abg_engine::TL_RUNS];
     CU(cudaEventSynchronize(ts[1]));
     CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
     return ABG_OK;

@@ -26,7 +26,11 @@ SYMBOLS = [
     "abg_debug_run_outputs", "abg_debug_k1_outputs", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
     "abg_carrier_configure", "abg_fetch_carrier", "abg_debug_carrier_time",
     "abg_input_meter_configure", "abg_fetch_input_levels", "abg_debug_input_meter_time",
+    "abg_subband_configure", "abg_fetch_subband", "abg_debug_subband_time",
 ]
+
+SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
+SUBBAND_MAX_COEFFS = 4096  # ABG_SUBBAND_MAX_COEFFS
 
 
 class COptions(C.Structure):
@@ -122,6 +126,10 @@ def load():
     L.abg_input_meter_configure.restype, L.abg_input_meter_configure.argtypes = i, [vp, i, i]
     L.abg_fetch_input_levels.restype, L.abg_fetch_input_levels.argtypes = i, [vp, i, C.POINTER(CInputLevels)]
     L.abg_debug_input_meter_time.restype, L.abg_debug_input_meter_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_subband_configure.restype, L.abg_subband_configure.argtypes = i, [vp, i, i, C.c_double, i, i, vp]
+    L.abg_fetch_subband.restype = i
+    L.abg_fetch_subband.argtypes = [vp, i, i, vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
+    L.abg_debug_subband_time.restype, L.abg_debug_subband_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -147,6 +155,7 @@ class Engine:
         self.h = h
         self.B = self.L.abg_wave_batch(self.h)
         self.nbmax = max_batches_per_run
+        self._sb_decim = {}  # (dev, k) -> smallest decimation configured: sizes fetch_subband's buffer
 
     def _chk(self, rc: int) -> int:
         if rc < 0:
@@ -356,6 +365,36 @@ class Engine:
         self._chk(self.L.abg_debug_input_meter_time(self.h, C.byref(ms)))
         return float(ms.value)
 
+    # ---- sub-band I/Q outputs ------------------------------------------------------------------------------------
+    def subband_configure(self, dev: int, k: int, offset_hz: float, decim: int, coeffs=None) -> None:
+        """Output k (0 .. SUBBAND_MAX-1) of a device: the band around offset_hz (from the centre frequency) mixed to 0 Hz,
+        filtered by the real FIR `coeffs` and decimated by `decim`, as cf32 (definition in airband_b200.h; `subband_lowpass`
+        designs a filter).  decim = 0 switches it off.  Applies to batches enqueued by later runs; a new configuration
+        restarts the output."""
+        if decim == 0:
+            self._chk(self.L.abg_subband_configure(self.h, dev, k, 0.0, 0, 0, None))
+            return
+        h = None if coeffs is None else np.ascontiguousarray(coeffs, dtype=np.float32)
+        self._chk(self.L.abg_subband_configure(self.h, dev, k, float(offset_hz), int(decim), 0 if h is None else h.size, _ptr(h)))
+        self._sb_decim[(dev, k)] = min(int(decim), self._sb_decim.get((dev, k), int(decim)))
+
+    def fetch_subband(self, dev: int, k: int) -> Optional[Tuple[np.ndarray, int, int]]:
+        """Oldest unfetched batch of output k: (complex64[n], batch_seq, first_index), first_index = m of its first
+        output; or None.  Lossy: at most max_batches_per_run + 2 are kept per output."""
+        n_in = self.B * self.cfg.hop(dev)
+        d = self._sb_decim.get((dev, k), 1)
+        buf = np.empty(2 * (-(-n_in // d)), np.float32)
+        seq, first, n = C.c_uint64(0), C.c_uint64(0), C.c_int32(0)
+        if not self._chk(self.L.abg_fetch_subband(self.h, dev, k, _ptr(buf), C.byref(seq), C.byref(first), C.byref(n))):
+            return None
+        return buf[:2 * n.value].view(np.complex64).copy(), int(seq.value), int(first.value)
+
+    def subband_time(self) -> float:
+        """ms of the sub-band kernel in the most recent run (CUDA events on the K1 stream); 0 if it computed nothing."""
+        ms = C.c_float(0.0)
+        self._chk(self.L.abg_debug_subband_time(self.h, C.byref(ms)))
+        return float(ms.value)
+
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
         """mixers[m] = [(dev, chan, ampfactor, balance), ...]"""
@@ -449,6 +488,33 @@ def input_levels(reading: dict) -> dict:
         skew = float(np.degrees(np.arcsin(np.clip(cov / np.sqrt(var[0] * var[1]), -1.0, 1.0))))
     return dict(dc_offset=mean, mean_square_dbfs=ms_db, full_scale_fraction=(h[:, 0] + h[:, 255]).astype(np.float64) / n,
                 codes_in_use=np.count_nonzero(h, axis=1), imbalance_db=imb, phase_skew_deg=skew)
+
+
+def subband_frequency(offset_hz: float, sample_rate: float) -> float:
+    """The frequency a sub-band output actually sits at, relative to the centre frequency: delta * sample_rate / 2^32
+    with delta = llround(offset_hz / sample_rate * 2^32) mod 2^32, folded into [-sample_rate/2, sample_rate/2)."""
+    x = float(offset_hz) / float(sample_rate) * 4294967296.0
+    r = int(np.floor(abs(x) + 0.5)) * (1 if x >= 0 else -1)  # llround: halves away from zero
+    delta = r % (1 << 32)
+    if delta >= 1 << 31:
+        delta -= 1 << 32
+    return delta * float(sample_rate) / 4294967296.0
+
+
+def subband_lowpass(n_coeffs: int, cutoff_hz: float, sample_rate: float, atten_db: float = 60.0) -> np.ndarray:
+    """Kaiser-windowed sinc low-pass for a sub-band output: float32[n_coeffs], the ideal sinc's edge at cutoff_hz, unit
+    gain at DC.  Kaiser's beta for a stopband atten_db below the passband; the stopband starts about
+    (atten_db - 7.95) / (14.36 * (n_coeffs - 1)) * sample_rate above the cutoff."""
+    if n_coeffs < 1 or n_coeffs > SUBBAND_MAX_COEFFS:
+        raise ValueError(f"n_coeffs must be in [1, {SUBBAND_MAX_COEFFS}]")
+    if not 0 < cutoff_hz <= sample_rate / 2:
+        raise ValueError("cutoff_hz must be in (0, sample_rate/2]")
+    a = float(atten_db)
+    beta = 0.1102 * (a - 8.7) if a > 50 else (0.5842 * (a - 21) ** 0.4 + 0.07886 * (a - 21) if a >= 21 else 0.0)
+    t = np.arange(n_coeffs, dtype=np.float64) - (n_coeffs - 1) / 2.0
+    fc = 2.0 * cutoff_hz / sample_rate
+    h = fc * np.sinc(fc * t) * np.kaiser(n_coeffs, beta)
+    return (h / h.sum()).astype(np.float32)
 
 
 TC_PLAN_FIELDS = ("eligible", "K", "HC", "S", "NC", "ND", "C2p", "KBS", "NSTB", "acc_regs", "smem_bytes", "halo", "consumer_warpgroups", "pps")
