@@ -168,14 +168,15 @@ struct DevBuf {
     }
 };
 
-// Result queue of one device's batch monitor (band spectrum, carrier meter, input level meter).  The monitor's kernel
-// writes the result of every batch straight into a page-locked, mapped ring of `cap` = max_batches_per_run + 2 entries;
-// the host keeps the unfetched entries, oldest first.  Lossy by design: queueing a run drops the oldest unfetched entries
-// beyond the ring's size (gaps show in their batch_seq), so a monitor never holds a result slot or causes ABG_EOVERFLOW.
+// Result queue of one device's batch monitor (band spectrum, carrier meter, input level meter, sub-band output).  The
+// monitor's kernel writes the result of every batch straight into a page-locked, mapped ring of `cap` =
+// max_batches_per_run + 2 entries; the host keeps the unfetched entries, oldest first.  Lossy by design: queueing a run
+// drops the oldest unfetched entries beyond the ring's size (gaps show in their batch_seq), so a monitor never holds a
+// result slot or causes ABG_EOVERFLOW.
 struct MonitorQueue {
     struct Entry {
-        int pos;           // ring entry
-        int32_t n_frames;  // monitor-specific count (spectrum: frames averaged)
+        int pos;      // ring entry
+        int32_t aux;  // monitor-specific: frames averaged (spectrum), decimation (sub-band output), 0 otherwise
         uint64_t seq, run;
     };
     unsigned char* ring = nullptr;  // [cap][entry_bytes]; allocated when the monitor is first switched on, kept until abg_destroy
@@ -214,13 +215,30 @@ struct MonitorQueue {
         return true;
     }
     // Queue the n batches of run `run` whose first is batch number seq0; returns the ring entry of the first.
-    int queue(int n, uint64_t seq0, uint64_t run, int32_t n_frames) {
+    int queue(int n, uint64_t seq0, uint64_t run, int32_t aux) {
         const int pos0 = next;
-        for (int b = 0; b < n; b++) ready.push_back({(next + b) % cap, n_frames, seq0 + (uint64_t)b, run});
+        for (int b = 0; b < n; b++) ready.push_back({(next + b) % cap, aux, seq0 + (uint64_t)b, run});
         while ((int)ready.size() > cap) ready.pop_front();
         next = (next + n) % cap;
         return pos0;
     }
+};
+
+constexpr int TL_RUNS = 8;  // runs whose timing events are kept
+
+// Host side of one batch monitor's launch: one kernel per run covers every device the monitor is on for.  The
+// sequence around it is shared (monitor_on, monitor_publish, monitor_launch, monitor_time); DESIGN.md §4, "Engine
+// plumbing", states its contract.
+template <typename Cfg, typename Run>
+struct MonitorLaunch {
+    const char* name;        // in error messages
+    bool reads_raw;          // reads raw[] after K1: records ev_raw, which abg_push's compaction waits for
+    std::vector<int> devs;   // covered devices in launch order (grid.y of the kernel)
+    DevBuf<Cfg> cfg;         // [devs.size()], written when a configure call changes the list
+    DevBuf<Run> run;         // room for every device, uploaded with every run
+    std::vector<Run> h_run;  // [devs.size()]
+    cudaEvent_t tl[TL_RUNS][2] = {};  // kernel start / end of the last TL_RUNS runs
+    bool ran[TL_RUNS] = {};
 };
 
 struct Device {
@@ -260,7 +278,7 @@ struct Device {
         uint32_t delta = 0;
         long long start = 0;         // absolute sample index of the output's first input sample
         float2* coef = nullptr;      // device [coef_cap]: h[j] * exp(+2 pi i delta j / 2^32); kept once allocated
-        MonitorQueue q;              // cf32 [ceil(n / decim)] per entry, Entry.n_frames = decim
+        MonitorQueue q;              // cf32 [ceil(n / decim)] per entry, Entry.aux = decim
     } sb[ABG_SUBBAND_MAX];
     int sb_hist = 0;                 // L_max - 1 over the outputs switched on: samples compaction keeps before `consumed`
     size_t dropped = 0;              // stream bytes compaction has dropped: raw[cur][0] is byte `dropped` of the stream
@@ -395,42 +413,18 @@ struct abg_engine {
     int k2_lpw = 32;
     uint64_t launches = 0;
     // timing events of the last TL_RUNS runs: [0] K1 start, [1] K1 end (stream A); [2] K2 start, [3] K2 end, [4] end of run (stream B)
-    static constexpr int TL_RUNS = 8;
     cudaEvent_t tl[TL_RUNS][5] = {};
     bool tev_valid = false;
     std::vector<int32_t> h_bins;
-    // band spectrum monitor
-    std::vector<int> spec_devs;              // monitored devices in launch order (grid.y of the spectrum kernel)
-    DevBuf<SpecCfg> spec_cfg;                // [spec_devs.size()]
-    DevBuf<SpecRun> spec_run;                // room for every device
-    std::vector<SpecRun> h_spec_run;
-    cudaEvent_t ev_raw[2] = {nullptr, nullptr};   // after the last kernel that read raw[] (K1 aside: the band spectrum, the
-                                                  // input meter, the sub-band outputs) of the latest run of each parity
-                                                  // that ran one
-    cudaEvent_t tl_spec[TL_RUNS][2] = {};    // spectrum kernel start / end of the last TL_RUNS runs
-    bool spec_ran[TL_RUNS] = {};
-    // carrier frequency meter
-    std::vector<int> car_devs;               // metered devices in launch order (grid.y of the meter kernel)
-    DevBuf<CarCfg> car_cfg;                  // [car_devs.size()]
-    DevBuf<CarRun> car_run;                  // room for every device
-    std::vector<CarRun> h_car_run;
-    cudaEvent_t tl_car[TL_RUNS][2] = {};     // meter kernel start / end of the last TL_RUNS runs
-    bool car_ran[TL_RUNS] = {};
-    // input level meter
-    std::vector<int> inm_devs;               // metered devices in launch order (grid.y of the meter kernel)
-    DevBuf<InmCfg> inm_cfg;                  // [inm_devs.size()]
-    DevBuf<InmRun> inm_run;                  // room for every device
-    std::vector<InmRun> h_inm_run;
-    cudaEvent_t tl_inm[TL_RUNS][2] = {};     // meter kernel start / end of the last TL_RUNS runs
-    bool inm_ran[TL_RUNS] = {};
-    // sub-band I/Q outputs
-    std::vector<int> sb_devs;                // devices with an output on, in launch order (grid.y of the kernel)
-    DevBuf<SbCfg> sb_cfg;                    // [sb_devs.size()]
-    DevBuf<SbRun> sb_run;                    // room for every device
-    std::vector<SbRun> h_sb_run;
-    int sb_max_hist = 0;                     // largest Device::sb_hist of sb_devs
-    cudaEvent_t tl_sb[TL_RUNS][2] = {};      // sub-band kernel start / end of the last TL_RUNS runs
-    bool sb_ran[TL_RUNS] = {};
+    // batch monitors, launched in this order on stream A after K1
+    MonitorLaunch<SpecCfg, SpecRun> spectrum{"spectrum", true};
+    MonitorLaunch<CarCfg, CarRun> carrier{"carrier meter", false};
+    MonitorLaunch<InmCfg, InmRun> input_meter{"input meter", true};
+    MonitorLaunch<SbCfg, SbRun> subband{"sub-band", true};
+    int sb_max_hist = 0;  // largest Device::sb_hist of subband.devs
+    // after the last monitor that read raw[] in the latest run of each parity that launched one; created when the first
+    // such monitor is switched on
+    cudaEvent_t ev_raw[2] = {nullptr, nullptr};
     // mixers (reference src/mixer.cpp)
     int n_mixers = 0;
     DevBuf<int32_t> mix_offsets;
@@ -455,6 +449,87 @@ struct abg_engine {
 
 namespace {
 
+// Switching a monitor on for its first device creates its timing events, and ev_raw if it reads raw[].
+template <typename Cfg, typename Run>
+int monitor_on(abg_engine* e, MonitorLaunch<Cfg, Run>& m) {
+    if (!m.tl[0][0])
+        for (auto& row : m.tl)
+            for (auto& ev : row) CU(cudaEventCreate(&ev));
+    if (m.reads_raw && !e->ev_raw[0])
+        for (int k = 0; k < 2; k++) CU(cudaEventCreateWithFlags(&e->ev_raw[k], cudaEventDisableTiming));
+    return ABG_OK;
+}
+
+// Install the device list and static table a configure call built.  With no device left nothing is allocated.
+template <typename Cfg, typename Run>
+int monitor_publish(abg_engine* e, MonitorLaunch<Cfg, Run>& m, const std::vector<int>& devs, const std::vector<Cfg>& cfgs) {
+    m.devs = devs;
+    m.cfg.free();
+    m.h_run.assign(devs.size(), Run{});
+    if (cfgs.empty()) return ABG_OK;
+    if (m.cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the %s tables", m.name);
+    CU(cudaMemcpy(m.cfg.p, cfgs.data(), sizeof(Cfg) * cfgs.size(), cudaMemcpyHostToDevice));
+    // upload_small writes whole 16-byte words: room for every device plus up to 15 bytes of rounding
+    if (!m.run.p && m.run.alloc(e->dev.size() + (15 + sizeof(Run) - 1) / sizeof(Run)))
+        return fail(ABG_ENOMEM, "Out of device memory for the %s tables", m.name);
+    return ABG_OK;
+}
+
+// One run of a monitor on stream A, after its h_run records are filled: their upload, then `kernel(n_devices,
+// max_items, stream)` between the timing events, then ev_raw if it reads raw[].  Nothing when max_items is 0.
+template <typename Cfg, typename Run, typename Kernel>
+int monitor_launch(abg_engine* e, MonitorLaunch<Cfg, Run>& m, int max_items, Kernel&& kernel) {
+    if (max_items <= 0) return ABG_OK;
+    cudaStream_t sa = e->stream;
+    const int t = (int)(e->run_index % TL_RUNS);
+    const int nl = upload_small(m.run.p, m.h_run.data(), sizeof(Run) * m.devs.size(), sa);
+    if (nl < 0) return fail(ABG_ECUDA, "%s parameter upload failed: %s", m.name, cudaGetErrorString(cudaGetLastError()));
+    e->launches += (uint64_t)nl;
+    CU(cudaEventRecord(m.tl[t][0], sa));
+    const cudaError_t er = kernel((int)m.devs.size(), max_items, sa);
+    if (er != cudaSuccess) return fail(ABG_ECUDA, "%s launch failed: %s", m.name, cudaGetErrorString(er));
+    e->launches++;
+    CU(cudaEventRecord(m.tl[t][1], sa));
+    if (m.reads_raw) CU(cudaEventRecord(e->ev_raw[e->run_index & 1], sa));
+    m.ran[t] = true;
+    return ABG_OK;
+}
+
+// ms of the monitor's kernel in the most recent run; 0 if that run did not launch it.  `fn` names the entry point.
+template <typename Cfg, typename Run>
+int monitor_time(abg_engine* e, const MonitorLaunch<Cfg, Run>& m, float* ms, const char* fn) {
+    if (!ms) return fail(ABG_EINVAL, "%s: null argument", fn);
+    *ms = 0.0f;
+    if (e->run_index == 0 || !m.ran[(e->run_index - 1) % TL_RUNS]) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    const cudaEvent_t* ts = m.tl[(e->run_index - 1) % TL_RUNS];
+    CU(cudaEventSynchronize(ts[1]));
+    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
+    return ABG_OK;
+}
+
+// Pop the oldest entry of one of monitor m's queues once m's kernel of the entry's run has finished: returns 1 and the
+// entry's ring bytes in *data, 0 if the queue is empty, < 0 on error.
+template <typename Cfg, typename Run>
+int monitor_pop(abg_engine* e, MonitorQueue& q, const MonitorLaunch<Cfg, Run>& m, const unsigned char** data, MonitorQueue::Entry* got) {
+    if (q.ready.empty()) return 0;
+    *got = q.ready.front();
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaEventSynchronize(m.tl[got->run % TL_RUNS][1]));  // (a later record of it is a later run: also fine)
+    *data = q.ring + (size_t)got->pos * q.entry_bytes;
+    q.ready.pop_front();  // the bytes stay put until a later run is enqueued
+    return 1;
+}
+
+template <typename Cfg, typename Run>
+void monitor_free(MonitorLaunch<Cfg, Run>& m) {
+    m.cfg.free();
+    m.run.free();
+    for (auto& row : m.tl)
+        for (auto& ev : row)
+            if (ev) cudaEventDestroy(ev);
+}
+
 void engine_free(abg_engine* e) {
     if (!e) return;
     cudaSetDevice(e->cuda_dev);
@@ -475,22 +550,10 @@ void engine_free(abg_engine* e) {
             so.q.release();
         }
     }
-    e->spec_cfg.free(); e->spec_run.free();
-    e->car_cfg.free(); e->car_run.free();
-    e->inm_cfg.free(); e->inm_run.free();
-    e->sb_cfg.free(); e->sb_run.free();
-    for (auto& row : e->tl_spec)
-        for (auto& ev : row)
-            if (ev) cudaEventDestroy(ev);
-    for (auto& row : e->tl_car)
-        for (auto& ev : row)
-            if (ev) cudaEventDestroy(ev);
-    for (auto& row : e->tl_inm)
-        for (auto& ev : row)
-            if (ev) cudaEventDestroy(ev);
-    for (auto& row : e->tl_sb)
-        for (auto& ev : row)
-            if (ev) cudaEventDestroy(ev);
+    monitor_free(e->spectrum);
+    monitor_free(e->carrier);
+    monitor_free(e->input_meter);
+    monitor_free(e->subband);
     for (auto& g : e->groups) {
         g.wsc.free();
         g.tc_btab.free(); g.tc_sq.free(); g.tc_tab_of_dev.free();
@@ -927,6 +990,13 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
     return ABG_OK;
 }
 
+// Byte of frame j = 0 of the run's first batch in the buffer K1 reads this run (the resident buffer is a stream of its
+// own): the first AGC_EXTRA frames of a stream only prime the AGC look-back.
+unsigned long long run_first_byte(const Device& d, bool resident) {
+    const unsigned long long look_back = (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes;
+    return resident ? look_back : (unsigned long long)d.consumed + (d.primed ? 0ull : look_back);
+}
+
 // enqueue K1 (+K2) for the per-device batch counts in nb[]; `resident` selects the replay buffers.
 int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool queue_outputs, int* n_enqueued, bool skip_k1 = false) {
     const int B = e->B, N = e->N;
@@ -957,7 +1027,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
         CU(cudaStreamWaitEvent(sa, e->ev_ingest, 0));
         e->ingest_dirty = false;
     }
-    cudaEvent_t* tl = e->tl[ri % abg_engine::TL_RUNS];
+    cudaEvent_t* tl = e->tl[ri % TL_RUNS];
     CU(cudaEventRecord(tl[0], sa));
     // ---- K1 per group (stream A) ----
     for (auto& g : e->groups) {
@@ -1009,117 +1079,69 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     }
     CU(cudaEventRecord(tl[1], sa));
     CU(cudaEventRecord(e->ev_k1[cur], sa));
-    // ---- band spectrum of the monitored devices (stream A: after K1, which K2 does not wait for past ev_k1) ----
-    e->spec_ran[ri % abg_engine::TL_RUNS] = false;
-    if (!skip_k1 && !e->spec_devs.empty()) {
+    // ---- batch monitors (stream A after K1 in this order: the spectrum, the carrier meter, the input meter, the sub-band
+    // outputs; K2 does not wait for them past ev_k1).  Injected batches have no frames and launch none. ----
+    const int t = (int)(ri % TL_RUNS);
+    e->spectrum.ran[t] = e->carrier.ran[t] = e->input_meter.ran[t] = e->subband.ran[t] = false;
+    if (!skip_k1) {
         int max_items = 0;
-        for (size_t m = 0; m < e->spec_devs.size(); m++) {
-            Device& d = e->dev[e->spec_devs[m]];
-            const int n = nb[e->spec_devs[m]];
-            SpecRun& r = e->h_spec_run[m];
-            const bool primed = resident ? d.res_primed : d.primed;
+        for (size_t m = 0; m < e->spectrum.devs.size(); m++) {
+            Device& d = e->dev[e->spectrum.devs[m]];
+            const int n = nb[e->spectrum.devs[m]];
+            SpecRun& r = e->spectrum.h_run[m];
             r.raw = resident ? d.res : d.raw[d.cur];
-            // frame j = 0 of the run's first batch: the first AGC_EXTRA frames of a stream only prime the AGC look-back
-            r.first_byte = resident ? (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes
-                                    : (unsigned long long)d.consumed + (primed ? 0ull : (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes);
+            r.first_byte = run_first_byte(d, resident);
             r.n_batches = n;
             r.ring_pos0 = queue_outputs && n > 0 ? d.spec_q.queue(n, d.batch_seq, ri, d.spec_n_sel) : -1;
             max_items = std::max(max_items, n * d.spec_chunks);
         }
-        if (max_items > 0) {
-            const int nl = upload_small(e->spec_run.p, e->h_spec_run.data(), sizeof(SpecRun) * e->spec_devs.size(), sa);
-            if (nl < 0) return fail(ABG_ECUDA, "spectrum parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-            e->launches += (uint64_t)nl;
+        int rc = monitor_launch(e, e->spectrum, max_items, [&](int n_devices, int items, cudaStream_t s) {
             SpecArgs A{};
-            A.cfg = e->spec_cfg.p; A.run = e->spec_run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
-            cudaEvent_t* ts = e->tl_spec[ri % abg_engine::TL_RUNS];
-            CU(cudaEventRecord(ts[0], sa));
-            cudaError_t ers = abg_launch_spectrum(N, A, (int)e->spec_devs.size(), max_items, sa);
-            if (ers != cudaSuccess) return fail(ABG_ECUDA, "spectrum launch failed: %s", cudaGetErrorString(ers));
-            e->launches++;
-            CU(cudaEventRecord(ts[1], sa));
-            CU(cudaEventRecord(e->ev_raw[cur], sa));
-            e->spec_ran[ri % abg_engine::TL_RUNS] = true;
-        }
-    }
-    // ---- carrier meter of the metered devices (stream A: after K1 and the spectrum; reads iqin[cur], which the next
-    // K1 to write it, two runs later, queues behind on this stream) ----
-    e->car_ran[ri % abg_engine::TL_RUNS] = false;
-    if (!skip_k1 && !e->car_devs.empty()) {
-        int max_items = 0;
-        for (size_t m = 0; m < e->car_devs.size(); m++) {
-            Device& d = e->dev[e->car_devs[m]];
-            const int n = nb[e->car_devs[m]];
-            CarRun& r = e->h_car_run[m];
+            A.cfg = e->spectrum.cfg.p; A.run = e->spectrum.run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
+            return abg_launch_spectrum(N, A, n_devices, items, s);
+        });
+        if (rc != ABG_OK) return rc;
+        // the carrier meter reads iqin[cur], which the next K1 to write it, two runs later, queues behind on this stream
+        max_items = 0;
+        for (size_t m = 0; m < e->carrier.devs.size(); m++) {
+            Device& d = e->dev[e->carrier.devs[m]];
+            const int n = nb[e->carrier.devs[m]];
+            CarRun& r = e->carrier.h_run[m];
             r.n_batches = n;
             r.ring_pos0 = queue_outputs && n > 0 ? d.car_q.queue(n, d.batch_seq, ri, 0) : -1;
             max_items = std::max(max_items, n * abg_carrier_items(d.C));
         }
-        if (max_items > 0) {
-            const int nl = upload_small(e->car_run.p, e->h_car_run.data(), sizeof(CarRun) * e->car_devs.size(), sa);
-            if (nl < 0) return fail(ABG_ECUDA, "carrier meter parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-            e->launches += (uint64_t)nl;
+        rc = monitor_launch(e, e->carrier, max_items, [&](int n_devices, int items, cudaStream_t s) {
             CarArgs A{};
-            A.cfg = e->car_cfg.p; A.run = e->car_run.p; A.iqin = e->iqin[cur].p; A.Gp = e->Gp; A.wave_batch = B;
-            cudaEvent_t* ts = e->tl_car[ri % abg_engine::TL_RUNS];
-            CU(cudaEventRecord(ts[0], sa));
-            cudaError_t erc = abg_launch_carrier(A, (int)e->car_devs.size(), max_items, sa);
-            if (erc != cudaSuccess) return fail(ABG_ECUDA, "carrier meter launch failed: %s", cudaGetErrorString(erc));
-            e->launches++;
-            CU(cudaEventRecord(ts[1], sa));
-            e->car_ran[ri % abg_engine::TL_RUNS] = true;
-        }
-    }
-    // ---- input level meter of the metered devices (stream A: after K1, the spectrum and the carrier meter; reads the
-    // raw bytes K1 read, so abg_push's compaction waits for it through ev_raw) ----
-    e->inm_ran[ri % abg_engine::TL_RUNS] = false;
-    if (!skip_k1 && !e->inm_devs.empty()) {
-        int max_items = 0;
-        for (size_t m = 0; m < e->inm_devs.size(); m++) {
-            Device& d = e->dev[e->inm_devs[m]];
-            const int n = nb[e->inm_devs[m]];
-            InmRun& r = e->h_inm_run[m];
-            const bool primed = resident ? d.res_primed : d.primed;
+            A.cfg = e->carrier.cfg.p; A.run = e->carrier.run.p; A.iqin = e->iqin[cur].p; A.Gp = e->Gp; A.wave_batch = B;
+            return abg_launch_carrier(A, n_devices, items, s);
+        });
+        if (rc != ABG_OK) return rc;
+        max_items = 0;
+        for (size_t m = 0; m < e->input_meter.devs.size(); m++) {
+            Device& d = e->dev[e->input_meter.devs[m]];
+            const int n = nb[e->input_meter.devs[m]];
+            InmRun& r = e->input_meter.h_run[m];
             r.raw = resident ? d.res : d.raw[d.cur];
-            // the same first byte as the spectrum's frame j = 0 of the run's first batch
-            r.first_byte = resident ? (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes
-                                    : (unsigned long long)d.consumed + (primed ? 0ull : (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes);
+            r.first_byte = run_first_byte(d, resident);
             r.n_batches = n;
             r.ring_pos0 = queue_outputs && n > 0 ? d.inm_q.queue(n, d.batch_seq, ri, 0) : -1;
             max_items = std::max(max_items, n * d.inm_chunks);
         }
-        if (max_items > 0) {
-            const int nl = upload_small(e->inm_run.p, e->h_inm_run.data(), sizeof(InmRun) * e->inm_devs.size(), sa);
-            if (nl < 0) return fail(ABG_ECUDA, "input meter parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-            e->launches += (uint64_t)nl;
+        rc = monitor_launch(e, e->input_meter, max_items, [&](int n_devices, int items, cudaStream_t s) {
             InmArgs A{};
-            A.cfg = e->inm_cfg.p; A.run = e->inm_run.p; A.wave_batch = B;
-            cudaEvent_t* ts = e->tl_inm[ri % abg_engine::TL_RUNS];
-            CU(cudaEventRecord(ts[0], sa));
-            cudaError_t eri = abg_launch_input_meter(A, (int)e->inm_devs.size(), max_items, sa);
-            if (eri != cudaSuccess) return fail(ABG_ECUDA, "input meter launch failed: %s", cudaGetErrorString(eri));
-            e->launches++;
-            CU(cudaEventRecord(ts[1], sa));
-            CU(cudaEventRecord(e->ev_raw[cur], sa));
-            e->inm_ran[ri % abg_engine::TL_RUNS] = true;
-        }
-    }
-    // ---- sub-band outputs of the devices with one on (stream A: after K1 and the monitors; reads raw[], so abg_push's
-    // compaction waits for it through ev_raw) ----
-    e->sb_ran[ri % abg_engine::TL_RUNS] = false;
-    if (!skip_k1 && !e->sb_devs.empty()) {
-        int max_items = 0;
-        for (size_t m = 0; m < e->sb_devs.size(); m++) {
-            Device& d = e->dev[e->sb_devs[m]];
-            const int n = nb[e->sb_devs[m]];
-            SbRun& r = e->h_sb_run[m];
-            const bool primed = resident ? d.res_primed : d.primed;
+            A.cfg = e->input_meter.cfg.p; A.run = e->input_meter.run.p; A.wave_batch = B;
+            return abg_launch_input_meter(A, n_devices, items, s);
+        });
+        if (rc != ABG_OK) return rc;
+        max_items = 0;
+        for (size_t m = 0; m < e->subband.devs.size(); m++) {
+            Device& d = e->dev[e->subband.devs[m]];
+            const int n = nb[e->subband.devs[m]];
+            SbRun& r = e->subband.h_run[m];
             r.raw = resident ? d.res : d.raw[d.cur];
-            // the input meter's first byte of the run's first batch; a resident buffer is a stream of its own
-            const unsigned long long first_byte = resident ? (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes
-                                                           : (unsigned long long)d.consumed + (primed ? 0ull : (unsigned long long)ABG_AGC_EXTRA * d.hop_bytes);
             r.base = resident ? 0 : (long long)(d.dropped / d.bpc);
-            r.s0 = r.base + (long long)(first_byte / d.bpc);
+            r.s0 = r.base + (long long)(run_first_byte(d, resident) / d.bpc);
             r.n_batches = n;
             int o = 0;
             for (auto& so : d.sb) {
@@ -1134,21 +1156,12 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             }
             max_items = std::max(max_items, n * abg_subband_chunks(B * d.hop));
         }
-        if (max_items > 0) {
-            const int nl = upload_small(e->sb_run.p, e->h_sb_run.data(), sizeof(SbRun) * e->sb_devs.size(), sa);
-            if (nl < 0) return fail(ABG_ECUDA, "sub-band parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-            e->launches += (uint64_t)nl;
+        rc = monitor_launch(e, e->subband, max_items, [&](int n_devices, int items, cudaStream_t s) {
             SbArgs A{};
-            A.cfg = e->sb_cfg.p; A.run = e->sb_run.p;
-            cudaEvent_t* ts = e->tl_sb[ri % abg_engine::TL_RUNS];
-            CU(cudaEventRecord(ts[0], sa));
-            cudaError_t ers = abg_launch_subband(A, (int)e->sb_devs.size(), max_items, e->sb_max_hist, sa);
-            if (ers != cudaSuccess) return fail(ABG_ECUDA, "sub-band launch failed: %s", cudaGetErrorString(ers));
-            e->launches++;
-            CU(cudaEventRecord(ts[1], sa));
-            CU(cudaEventRecord(e->ev_raw[cur], sa));
-            e->sb_ran[ri % abg_engine::TL_RUNS] = true;
-        }
+            A.cfg = e->subband.cfg.p; A.run = e->subband.run.p;
+            return abg_launch_subband(A, n_devices, items, e->sb_max_hist, s);
+        });
+        if (rc != ABG_OK) return rc;
     }
     // ---- K2 (stream B, after this run's K1; overlaps the next run's K1) ----
     CU(cudaStreamWaitEvent(sb, e->ev_k1[cur], 0));
@@ -1464,13 +1477,6 @@ int abg_fft_path(const abg_engine* e, int dev) {
     return g.use_tc ? 3 : (g.pruned ? 2 : 1);
 }
 
-// The monitors that read raw[] after K1 (band spectrum, input meter, sub-band outputs) record ev_raw, which abg_push's compaction waits for.
-static int create_raw_events(abg_engine* e) {
-    if (e->ev_raw[0]) return ABG_OK;
-    for (int k = 0; k < 2; k++) CU(cudaEventCreateWithFlags(&e->ev_raw[k], cudaEventDisableTiming));
-    return ABG_OK;
-}
-
 // ---- band spectrum monitor (definition in airband_b200.h) -------------------------------------------------------------
 int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_spectrum_configure: device %d out of range", dev);
@@ -1484,11 +1490,7 @@ int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
     d.spec_work = nullptr;
     d.spec_stride = d.spec_n_sel = d.spec_chunks = 0;
     if (frame_stride > 0) {
-        if (!e->tl_spec[0][0]) {
-            for (auto& row : e->tl_spec)
-                for (auto& ev : row) CU(cudaEventCreate(&ev));
-        }
-        if (create_raw_events(e) != ABG_OK) return ABG_ECUDA;
+        if (monitor_on(e, e->spectrum) != ABG_OK) return ABG_ECUDA;
         if (!d.spec_q.alloc(nbmax + 2, sizeof(float) * N)) return fail(ABG_ENOMEM, "Out of page-locked host memory for the spectrum ring");
         const int n_sel = (B + frame_stride - 1) / frame_stride;
         const int chunks = (n_sel + ABG_SPEC_FPC - 1) / ABG_SPEC_FPC;
@@ -1503,7 +1505,7 @@ int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
         d.spec_chunks = chunks;
     }
     // rebuild the launch's device list and its static table
-    e->spec_devs.clear();
+    std::vector<int> devs;
     std::vector<SpecCfg> cfgs;
     for (int i = 0; i < (int)e->dev.size(); i++) {
         const Device& x = e->dev[i];
@@ -1515,54 +1517,25 @@ int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
         CU(cudaHostGetDevicePointer((void**)&c.ring, x.spec_q.ring, 0));
         c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = x.spec_stride; c.n_sel = x.spec_n_sel; c.n_chunks = x.spec_chunks;
         c.ring_cap = nbmax + 2;
-        e->spec_devs.push_back(i);
+        devs.push_back(i);
         cfgs.push_back(c);
     }
-    e->spec_cfg.free();
-    e->h_spec_run.assign(e->spec_devs.size(), SpecRun{});
-    if (cfgs.empty()) return ABG_OK;
-    if (e->spec_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the spectrum tables");
-    CU(cudaMemcpy(e->spec_cfg.p, cfgs.data(), sizeof(SpecCfg) * cfgs.size(), cudaMemcpyHostToDevice));
-    // upload_small writes whole 16-byte words: room for every device plus the rounding
-    if (!e->spec_run.p && e->spec_run.alloc(e->dev.size() + 1)) return fail(ABG_ENOMEM, "Out of device memory for the spectrum tables");
-    return ABG_OK;
-}
-
-// Pop the oldest entry of a monitor queue once the monitor kernel of its run (end events `ends`) has finished: returns 1
-// and the entry's ring bytes in *data, 0 if the queue is empty, < 0 on error.
-static int monitor_pop(abg_engine* e, MonitorQueue& q, cudaEvent_t (&ends)[abg_engine::TL_RUNS][2], const unsigned char** data,
-                       MonitorQueue::Entry* got) {
-    if (q.ready.empty()) return 0;
-    *got = q.ready.front();
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaEventSynchronize(ends[got->run % abg_engine::TL_RUNS][1]));  // (a later record of it is a later run: also fine)
-    *data = q.ring + (size_t)got->pos * q.entry_bytes;
-    q.ready.pop_front();  // the bytes stay put until a later run is enqueued
-    return 1;
+    return monitor_publish(e, e->spectrum, devs, cfgs);
 }
 
 int abg_fetch_spectrum(abg_engine* e, int dev, float* power, uint64_t* batch_seq, int32_t* n_frames) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_spectrum: device %d out of range", dev);
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int rc = monitor_pop(e, e->dev[dev].spec_q, e->tl_spec, &src, &r);
+    const int rc = monitor_pop(e, e->dev[dev].spec_q, e->spectrum, &src, &r);
     if (rc <= 0) return rc;
     if (power) memcpy(power, src, sizeof(float) * e->N);
     if (batch_seq) *batch_seq = r.seq;
-    if (n_frames) *n_frames = r.n_frames;
+    if (n_frames) *n_frames = r.aux;
     return 1;
 }
 
-int abg_debug_spectrum_time(abg_engine* e, float* ms) {
-    if (!ms) return fail(ABG_EINVAL, "abg_debug_spectrum_time: null argument");
-    *ms = 0.0f;
-    if (e->run_index == 0 || !e->spec_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    cudaEvent_t* ts = e->tl_spec[(e->run_index - 1) % abg_engine::TL_RUNS];
-    CU(cudaEventSynchronize(ts[1]));
-    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
-    return ABG_OK;
-}
+int abg_debug_spectrum_time(abg_engine* e, float* ms) { return monitor_time(e, e->spectrum, ms, __func__); }
 
 // ---- carrier frequency meter (definition in airband_b200.h) -----------------------------------------------------------
 int abg_carrier_configure(abg_engine* e, int dev, int on) {
@@ -1573,14 +1546,12 @@ int abg_carrier_configure(abg_engine* e, int dev, int on) {
     cudaSetDevice(e->cuda_dev);
     CU(cudaStreamSynchronize(e->stream));  // an enqueued meter kernel may still read the device table
     if (on) {
-        if (!e->tl_car[0][0])
-            for (auto& row : e->tl_car)
-                for (auto& ev : row) CU(cudaEventCreate(&ev));
+        if (monitor_on(e, e->carrier) != ABG_OK) return ABG_ECUDA;
         if (!d.car_q.alloc(e->nbmax + 2, sizeof(float) * 3 * (size_t)std::max(d.C, 1))) return fail(ABG_ENOMEM, "Out of page-locked host memory for the carrier meter ring");
     }
     d.car_on = on == 1;
     // rebuild the launch's device list and its static table
-    e->car_devs.clear();
+    std::vector<int> devs;
     std::vector<CarCfg> cfgs;
     for (int i = 0; i < (int)e->dev.size(); i++) {
         const Device& x = e->dev[i];
@@ -1588,17 +1559,10 @@ int abg_carrier_configure(abg_engine* e, int dev, int on) {
         CarCfg c{};
         CU(cudaHostGetDevicePointer((void**)&c.ring, x.car_q.ring, 0));
         c.g0 = x.g0; c.n_channels = x.C; c.ring_cap = x.car_q.cap;
-        e->car_devs.push_back(i);
+        devs.push_back(i);
         cfgs.push_back(c);
     }
-    e->car_cfg.free();
-    e->h_car_run.assign(e->car_devs.size(), CarRun{});
-    if (cfgs.empty()) return ABG_OK;
-    if (e->car_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the carrier meter tables");
-    CU(cudaMemcpy(e->car_cfg.p, cfgs.data(), sizeof(CarCfg) * cfgs.size(), cudaMemcpyHostToDevice));
-    // upload_small writes whole 16-byte words: room for every device plus the rounding
-    if (!e->car_run.p && e->car_run.alloc(e->dev.size() + 2)) return fail(ABG_ENOMEM, "Out of device memory for the carrier meter tables");
-    return ABG_OK;
+    return monitor_publish(e, e->carrier, devs, cfgs);
 }
 
 int abg_fetch_carrier(abg_engine* e, int dev, float* lag1, float* energy, uint64_t* batch_seq) {
@@ -1606,7 +1570,7 @@ int abg_fetch_carrier(abg_engine* e, int dev, float* lag1, float* energy, uint64
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
     const int C = e->dev[dev].C;
-    const int rc = monitor_pop(e, e->dev[dev].car_q, e->tl_car, &src, &r);
+    const int rc = monitor_pop(e, e->dev[dev].car_q, e->carrier, &src, &r);
     if (rc <= 0) return rc;
     if (lag1) memcpy(lag1, src, sizeof(float) * 2 * C);
     if (energy) memcpy(energy, src + sizeof(float) * 2 * C, sizeof(float) * C);
@@ -1614,16 +1578,7 @@ int abg_fetch_carrier(abg_engine* e, int dev, float* lag1, float* energy, uint64
     return 1;
 }
 
-int abg_debug_carrier_time(abg_engine* e, float* ms) {
-    if (!ms) return fail(ABG_EINVAL, "abg_debug_carrier_time: null argument");
-    *ms = 0.0f;
-    if (e->run_index == 0 || !e->car_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    cudaEvent_t* ts = e->tl_car[(e->run_index - 1) % abg_engine::TL_RUNS];
-    CU(cudaEventSynchronize(ts[1]));
-    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
-    return ABG_OK;
-}
+int abg_debug_carrier_time(abg_engine* e, float* ms) { return monitor_time(e, e->carrier, ms, __func__); }
 
 // ---- input level meter (definition in airband_b200.h) -----------------------------------------------------------------
 int abg_input_meter_configure(abg_engine* e, int dev, int on) {
@@ -1638,10 +1593,7 @@ int abg_input_meter_configure(abg_engine* e, int dev, int on) {
     const size_t hist_bytes = sizeof(uint32_t) * 512 * (size_t)nbmax, counter_bytes = sizeof(int32_t) * (size_t)nbmax;
     const size_t part_off = (hist_bytes + counter_bytes + 15) & ~(size_t)15;
     if (on) {
-        if (!e->tl_inm[0][0])
-            for (auto& row : e->tl_inm)
-                for (auto& ev : row) CU(cudaEventCreate(&ev));
-        if (create_raw_events(e) != ABG_OK) return ABG_ECUDA;
+        if (monitor_on(e, e->input_meter) != ABG_OK) return ABG_ECUDA;
         if (!d.inm_q.alloc(nbmax + 2, sizeof(abg_input_levels))) return fail(ABG_ENOMEM, "Out of page-locked host memory for the input meter ring");
         if (!d.inm_work) {
             // histograms and counters start at zero; every launch leaves them at zero again
@@ -1655,7 +1607,7 @@ int abg_input_meter_configure(abg_engine* e, int dev, int on) {
     }
     d.inm_on = on == 1;
     // rebuild the launch's device list and its static table
-    e->inm_devs.clear();
+    std::vector<int> devs;
     std::vector<InmCfg> cfgs;
     for (int i = 0; i < (int)e->dev.size(); i++) {
         const Device& x = e->dev[i];
@@ -1668,24 +1620,17 @@ int abg_input_meter_configure(abg_engine* e, int dev, int on) {
         c.partial = reinterpret_cast<long long*>(w + part_off);
         c.sfmt = x.sfmt; c.hop_bytes = x.hop_bytes; c.n_chunks = x.inm_chunks; c.ring_cap = x.inm_q.cap;
         c.scale = 1.0f / x.fullscale;
-        e->inm_devs.push_back(i);
+        devs.push_back(i);
         cfgs.push_back(c);
     }
-    e->inm_cfg.free();
-    e->h_inm_run.assign(e->inm_devs.size(), InmRun{});
-    if (cfgs.empty()) return ABG_OK;
-    if (e->inm_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the input meter tables");
-    CU(cudaMemcpy(e->inm_cfg.p, cfgs.data(), sizeof(InmCfg) * cfgs.size(), cudaMemcpyHostToDevice));
-    // upload_small writes whole 16-byte words: room for every device plus the rounding
-    if (!e->inm_run.p && e->inm_run.alloc(e->dev.size() + 1)) return fail(ABG_ENOMEM, "Out of device memory for the input meter tables");
-    return ABG_OK;
+    return monitor_publish(e, e->input_meter, devs, cfgs);
 }
 
 int abg_fetch_input_levels(abg_engine* e, int dev, abg_input_levels* out) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_input_levels: device %d out of range", dev);
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int rc = monitor_pop(e, e->dev[dev].inm_q, e->tl_inm, &src, &r);
+    const int rc = monitor_pop(e, e->dev[dev].inm_q, e->input_meter, &src, &r);
     if (rc <= 0) return rc;
     if (out) {
         memcpy(out, src, sizeof(abg_input_levels));
@@ -1694,16 +1639,7 @@ int abg_fetch_input_levels(abg_engine* e, int dev, abg_input_levels* out) {
     return 1;
 }
 
-int abg_debug_input_meter_time(abg_engine* e, float* ms) {
-    if (!ms) return fail(ABG_EINVAL, "abg_debug_input_meter_time: null argument");
-    *ms = 0.0f;
-    if (e->run_index == 0 || !e->inm_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    cudaEvent_t* ts = e->tl_inm[(e->run_index - 1) % abg_engine::TL_RUNS];
-    CU(cudaEventSynchronize(ts[1]));
-    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
-    return ABG_OK;
-}
+int abg_debug_input_meter_time(abg_engine* e, float* ms) { return monitor_time(e, e->input_meter, ms, __func__); }
 
 // ---- sub-band I/Q outputs (definition in airband_b200.h) ---------------------------------------------------------------
 int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int decim, int n_coeffs, const float* coeffs) {
@@ -1726,10 +1662,7 @@ int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int d
     cudaSetDevice(e->cuda_dev);
     CU(cudaStreamSynchronize(e->stream));  // an enqueued kernel may still read the tables, the coefficients or the ring
     if (decim > 0) {
-        if (!e->tl_sb[0][0])
-            for (auto& row : e->tl_sb)
-                for (auto& ev : row) CU(cudaEventCreate(&ev));
-        if (create_raw_events(e) != ABG_OK) return ABG_ECUDA;
+        if (monitor_on(e, e->subband) != ABG_OK) return ABG_ECUDA;
         // delta = llround(offset / fs * 2^32) mod 2^32; g[j] = h[j] exp(+2 pi i delta j / 2^32) in double, then float32
         const uint32_t delta = (uint32_t)(unsigned long long)llround(offset_hz / d.sample_rate * 4294967296.0);
         std::vector<float2> g(n_coeffs);
@@ -1761,7 +1694,7 @@ int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int d
     for (const auto& x : d.sb)
         if (x.on) d.sb_hist = std::max(d.sb_hist, x.n_coeffs - 1);
     // rebuild the launch's device list and its static table
-    e->sb_devs.clear();
+    std::vector<int> devs;
     e->sb_max_hist = 0;
     std::vector<SbCfg> cfgs;
     for (int i = 0; i < (int)e->dev.size(); i++) {
@@ -1780,17 +1713,10 @@ int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int d
         c.hist = x.sb_hist;
         c.scale = 1.0f / x.fullscale;
         e->sb_max_hist = std::max(e->sb_max_hist, x.sb_hist);
-        e->sb_devs.push_back(i);
+        devs.push_back(i);
         cfgs.push_back(c);
     }
-    e->sb_cfg.free();
-    e->h_sb_run.assign(e->sb_devs.size(), SbRun{});
-    if (cfgs.empty()) return ABG_OK;
-    if (e->sb_cfg.alloc(cfgs.size())) return fail(ABG_ENOMEM, "Out of device memory for the sub-band tables");
-    CU(cudaMemcpy(e->sb_cfg.p, cfgs.data(), sizeof(SbCfg) * cfgs.size(), cudaMemcpyHostToDevice));
-    // upload_small writes whole 16-byte words: room for every device plus the rounding
-    if (!e->sb_run.p && e->sb_run.alloc(e->dev.size() + 1)) return fail(ABG_ENOMEM, "Out of device memory for the sub-band tables");
-    return ABG_OK;
+    return monitor_publish(e, e->subband, devs, cfgs);
 }
 
 int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t* batch_seq, uint64_t* first_index, int32_t* n_samples) {
@@ -1799,10 +1725,10 @@ int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t* batch_
     const Device& d = e->dev[dev];
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int rc = monitor_pop(e, e->dev[dev].sb[k].q, e->tl_sb, &src, &r);
+    const int rc = monitor_pop(e, e->dev[dev].sb[k].q, e->subband, &src, &r);
     if (rc <= 0) return rc;
     // the batch's outputs: s0 <= mD < s0 + n with D the decimation the batch was computed with
-    const unsigned long long n = (unsigned long long)e->B * d.hop, D = (unsigned long long)r.n_frames;
+    const unsigned long long n = (unsigned long long)e->B * d.hop, D = (unsigned long long)r.aux;
     const unsigned long long s0 = ((unsigned long long)ABG_AGC_EXTRA + r.seq * e->B) * d.hop;
     const unsigned long long m0 = (s0 + D - 1) / D, m1 = (s0 + n + D - 1) / D;
     if (iq) memcpy(iq, src, sizeof(float2) * (m1 - m0));
@@ -1812,16 +1738,7 @@ int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t* batch_
     return 1;
 }
 
-int abg_debug_subband_time(abg_engine* e, float* ms) {
-    if (!ms) return fail(ABG_EINVAL, "abg_debug_subband_time: null argument");
-    *ms = 0.0f;
-    if (e->run_index == 0 || !e->sb_ran[(e->run_index - 1) % abg_engine::TL_RUNS]) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    cudaEvent_t* ts = e->tl_sb[(e->run_index - 1) % abg_engine::TL_RUNS];
-    CU(cudaEventSynchronize(ts[1]));
-    CU(cudaEventElapsedTime(ms, ts[0], ts[1]));
-    return ABG_OK;
-}
+int abg_debug_subband_time(abg_engine* e, float* ms) { return monitor_time(e, e->subband, ms, __func__); }
 
 // ---- scan mode -------------------------------------------------------------------------------------------------------
 static ScanView scan_view(abg_engine* e) {
@@ -1975,7 +1892,7 @@ uint64_t abg_launch_count(const abg_engine* e) { return e->launches; }
 int abg_last_run_times(abg_engine* e, float* ms4) {
     if (!e->tev_valid) return fail(ABG_EINVAL, "abg_last_run_times: no run yet");
     cudaSetDevice(e->cuda_dev);
-    cudaEvent_t* tl = e->tl[(e->run_index - 1) % abg_engine::TL_RUNS];
+    cudaEvent_t* tl = e->tl[(e->run_index - 1) % TL_RUNS];
     CU(cudaEventSynchronize(tl[4]));
     CU(cudaEventElapsedTime(&ms4[0], tl[0], tl[1]));  // K1 on stream A
     CU(cudaEventElapsedTime(&ms4[1], tl[2], tl[3]));  // K2 on stream B
@@ -1987,14 +1904,14 @@ int abg_last_run_times(abg_engine* e, float* ms4) {
 // Timeline of the last n_runs (<= 8) runs: 5 timestamps per run (K1 start, K1 end, K2 start, K2 end, end of run) in ms
 // relative to the oldest run's K1 start.  Measurement aid: shows how runs overlap inside the stream pipeline.
 int abg_debug_timeline(abg_engine* e, int n_runs, float* ms) {
-    if (!ms || n_runs < 1 || n_runs > abg_engine::TL_RUNS || (uint64_t)n_runs > e->run_index)
+    if (!ms || n_runs < 1 || n_runs > TL_RUNS || (uint64_t)n_runs > e->run_index)
         return fail(ABG_EINVAL, "abg_debug_timeline: bad arguments");
     cudaSetDevice(e->cuda_dev);
-    cudaEvent_t* last = e->tl[(e->run_index - 1) % abg_engine::TL_RUNS];
+    cudaEvent_t* last = e->tl[(e->run_index - 1) % TL_RUNS];
     CU(cudaEventSynchronize(last[4]));
-    cudaEvent_t origin = e->tl[(e->run_index - n_runs) % abg_engine::TL_RUNS][0];
+    cudaEvent_t origin = e->tl[(e->run_index - n_runs) % TL_RUNS][0];
     for (int r = 0; r < n_runs; r++) {
-        cudaEvent_t* tl = e->tl[(e->run_index - n_runs + r) % abg_engine::TL_RUNS];
+        cudaEvent_t* tl = e->tl[(e->run_index - n_runs + r) % TL_RUNS];
         for (int k = 0; k < 5; k++) CU(cudaEventElapsedTime(&ms[r * 5 + k], origin, tl[k]));
     }
     return ABG_OK;

@@ -298,6 +298,12 @@ class Engine:
     def launch_count(self) -> int:
         return int(self.L.abg_launch_count(self.h))
 
+    def _kernel_time(self, debug_time) -> float:
+        """ms between a monitor kernel's CUDA events in the most recent run, from its abg_debug_*_time."""
+        ms = C.c_float(0.0)
+        self._chk(debug_time(self.h, C.byref(ms)))
+        return float(ms.value)
+
     # ---- band spectrum monitor -----------------------------------------------------------------------------------
     def spectrum_configure(self, dev: int, stride: int) -> None:
         """Batch-averaged power spectrum of a device every `stride`-th frame of each batch (0 = off, the default); applies
@@ -315,9 +321,7 @@ class Engine:
 
     def spectrum_time(self) -> float:
         """ms of the spectrum kernel in the most recent run (CUDA events on the K1 stream); 0 if it computed none."""
-        ms = C.c_float(0.0)
-        self._chk(self.L.abg_debug_spectrum_time(self.h, C.byref(ms)))
-        return float(ms.value)
+        return self._kernel_time(self.L.abg_debug_spectrum_time)
 
     # ---- carrier frequency meter ---------------------------------------------------------------------------------
     def carrier_configure(self, dev: int, on: bool) -> None:
@@ -338,9 +342,7 @@ class Engine:
 
     def carrier_time(self) -> float:
         """ms of the carrier meter kernel in the most recent run (CUDA events on the K1 stream); 0 if it metered nothing."""
-        ms = C.c_float(0.0)
-        self._chk(self.L.abg_debug_carrier_time(self.h, C.byref(ms)))
-        return float(ms.value)
+        return self._kernel_time(self.L.abg_debug_carrier_time)
 
     # ---- input level meter ---------------------------------------------------------------------------------------
     def input_meter_configure(self, dev: int, on: bool) -> None:
@@ -361,9 +363,7 @@ class Engine:
 
     def input_meter_time(self) -> float:
         """ms of the input meter kernel in the most recent run (CUDA events on the K1 stream); 0 if it metered nothing."""
-        ms = C.c_float(0.0)
-        self._chk(self.L.abg_debug_input_meter_time(self.h, C.byref(ms)))
-        return float(ms.value)
+        return self._kernel_time(self.L.abg_debug_input_meter_time)
 
     # ---- sub-band I/Q outputs ------------------------------------------------------------------------------------
     def subband_configure(self, dev: int, k: int, offset_hz: float, decim: int, coeffs=None) -> None:
@@ -391,9 +391,7 @@ class Engine:
 
     def subband_time(self) -> float:
         """ms of the sub-band kernel in the most recent run (CUDA events on the K1 stream); 0 if it computed nothing."""
-        ms = C.c_float(0.0)
-        self._chk(self.L.abg_debug_subband_time(self.h, C.byref(ms)))
-        return float(ms.value)
+        return self._kernel_time(self.L.abg_debug_subband_time)
 
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
