@@ -394,6 +394,12 @@ ABG_API int abg_debug_run_outputs(abg_engine* e, int32_t* dims, float* wout, uns
  * batches is its frame AGC_EXTRA + (batches before the run) * WAVE_BATCH + j for j < n * WAVE_BATCH and stale beyond.  K2 never
  * writes these rows, so closed-squelch stretches are visible here.  Waits for the run; either pointer may be NULL. */
 ABG_API int abg_debug_k1_outputs(abg_engine* e, int32_t* dims, float* win, float* iqin);
+/* The full spectra K1 of the device's most recent launch kept for AFC (K2's AFC block reads them, and only reads them):
+ * out float[n_rows][fft_size][2], natural bin order.  Row b is the spectrum of the last frame of the run's batch b, the
+ * frame whose iqin row is (b + 1) * WAVE_BATCH - 1 in abg_debug_k1_outputs; its value at a channel's bin is that row's
+ * iqin bit for bit.  *n_rows = batches of that launch (0 if the device had none).  ABG_EINVAL for a device without an AFC
+ * channel or before any run.  Waits for the run; out may be NULL to query n_rows. */
+ABG_API int abg_debug_k1_spectra(abg_engine* e, int dev, int32_t* n_rows, float* out);
 /* Feed |X[bin]| values straight into the demodulation state machine of one device (K1 skipped): wavein[C][n_batches *
  * WAVE_BATCH] becomes channel_t.wavein[AGC_EXTRA ...], and iq_in[C][n_batches * WAVE_BATCH][2] (may be NULL) the X[bin]
  * values of the same frames (channel_t.iq_in, where K1 would have stored them); results are fetched as usual.  For the

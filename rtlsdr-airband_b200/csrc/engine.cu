@@ -2086,6 +2086,25 @@ int abg_debug_k1_outputs(abg_engine* e, int32_t* dims, float* win, float* iqin) 
     return ABG_OK;
 }
 
+// see airband_b200.h: the Device::spec rows the device's most recent K1 launch wrote.  Its K1Dev record stays on the host
+// after the upload; row b is the frame at spec_first_pos + b * B, so the launch wrote the rows whose frame it computed.
+int abg_debug_k1_spectra(abg_engine* e, int dev, int32_t* n_rows, float* out) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_debug_k1_spectra: device %d out of range", dev);
+    const Device& d = e->dev[dev];
+    if (!d.has_afc) return fail(ABG_EINVAL, "abg_debug_k1_spectra: device %d has no AFC channel, so K1 keeps no spectrum", dev);
+    if (e->run_index == 0) return fail(ABG_EINVAL, "abg_debug_k1_spectra: nothing has run yet");
+    const Group& g = e->groups[d.group];
+    const size_t k = std::find(g.devs.begin(), g.devs.end(), dev) - g.devs.begin();
+    const K1Dev& a = g.h_k1[k];
+    const int rows = a.n_frames > 0 ? (a.pos0 + a.n_frames - a.spec_first_pos + a.wave_batch - 1) / a.wave_batch : 0;
+    if (n_rows) *n_rows = rows;
+    if (!out || rows == 0) return ABG_OK;
+    int rc = abg_sync(e);
+    if (rc != ABG_OK) return rc;
+    CU(cudaMemcpy(out, d.spec, sizeof(float2) * (size_t)rows * e->N, cudaMemcpyDeviceToHost));
+    return ABG_OK;
+}
+
 int abg_debug_frame(abg_engine* e, int dev, const void* iq_frame, float* fftout) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_debug_frame: device %d out of range", dev);
     cudaSetDevice(e->cuda_dev);

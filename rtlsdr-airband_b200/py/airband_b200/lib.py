@@ -23,7 +23,7 @@ SYMBOLS = [
     "abg_batches_available", "abg_run", "abg_sync", "abg_join", "abg_batches_ready", "abg_fetch_batch", "abg_fetch_batches", "abg_get_stats", "abg_set_bin",
     "abg_resident_load", "abg_run_resident", "abg_set_stream", "abg_launch_count", "abg_mixers_configure",
     "abg_fetch_mixer_batch", "abg_mixer_device_buffers", "abg_debug_frame", "abg_last_run_times", "abg_debug_timeline", "abg_scan_configure", "abg_scan_select", "abg_host_register", "abg_host_unregister", "abg_ingest_sync", "abg_fft_path", "abg_debug_tc_table", "abg_debug_inject_wavein", "abg_debug_k1tc_trace", "abg_debug_k2_stats",
-    "abg_debug_run_outputs", "abg_debug_k1_outputs", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
+    "abg_debug_run_outputs", "abg_debug_k1_outputs", "abg_debug_k1_spectra", "abg_spectrum_configure", "abg_fetch_spectrum", "abg_debug_spectrum_time",
     "abg_carrier_configure", "abg_fetch_carrier", "abg_debug_carrier_time",
     "abg_input_meter_configure", "abg_fetch_input_levels", "abg_debug_input_meter_time",
     "abg_subband_configure", "abg_fetch_subband", "abg_debug_subband_time",
@@ -105,6 +105,7 @@ def load():
     L.abg_debug_frame.restype, L.abg_debug_frame.argtypes = i, [vp, i, vp, vp]
     L.abg_debug_run_outputs.restype, L.abg_debug_run_outputs.argtypes = i, [vp, vp, vp, vp]
     L.abg_debug_k1_outputs.restype, L.abg_debug_k1_outputs.argtypes = i, [vp, vp, vp, vp]
+    L.abg_debug_k1_spectra.restype, L.abg_debug_k1_spectra.argtypes = i, [vp, i, vp, vp]
     L.abg_last_run_times.restype, L.abg_last_run_times.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_host_register.restype, L.abg_host_register.argtypes = i, [vp, C.c_size_t]
     L.abg_host_unregister.restype, L.abg_host_unregister.argtypes = i, [vp]
@@ -270,6 +271,15 @@ class Engine:
         iqin = np.empty((rows, 2 * Gp), np.float32)
         self._chk(self.L.abg_debug_k1_outputs(self.h, _ptr(dims), _ptr(win), _ptr(iqin)))
         return win[:, :G], iqin.view(np.complex64)[:, :G]
+
+    def k1_spectra(self, dev: int) -> np.ndarray:
+        """complex64 [batches, fft_size]: the full spectrum of each batch-final frame that K1 of the device's most recent launch
+        kept for AFC, natural bin order (abg_debug_k1_spectra; devices with an AFC channel only)."""
+        n = np.zeros(1, np.int32)
+        self._chk(self.L.abg_debug_k1_spectra(self.h, dev, _ptr(n), None))
+        out = np.empty((int(n[0]), 2 * self.cfg.fft_size), np.float32)
+        self._chk(self.L.abg_debug_k1_spectra(self.h, dev, _ptr(n), _ptr(out) if out.size else None))
+        return out.view(np.complex64)
 
     def set_stream(self, cuda_stream_ptr: int) -> None:
         self._chk(self.L.abg_set_stream(self.h, C.c_void_p(cuda_stream_ptr)))

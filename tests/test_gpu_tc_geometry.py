@@ -27,18 +27,23 @@ def sm_count():
 
 
 class Group:
-    """Devices of one sample format and hop (one K1 launch group) with different channel lists, streams and lengths."""
+    """Devices of one sample format, hop and fullscale (one K1 launch group) with different channel lists, streams and
+    lengths.  hop_bytes counts bytes between frames; `afc` lists devices whose channels use AFC."""
 
-    def __init__(self, n, hop_bytes, sfmt, bin_lists, batches, wave_rate=8000, seed0=0, streams=None):
+    def __init__(self, n, hop_bytes, sfmt, bin_lists, batches, wave_rate=8000, seed0=0, streams=None, fullscale=0.0, rails=False,
+                 afc=()):
         self.n, self.hop_bytes, self.sfmt, self.bin_lists, self.batches = n, hop_bytes, sfmt, [list(b) for b in bin_lists], list(batches)
         self.B = wave_rate // 8
-        sr = (hop_bytes // 2) * wave_rate
-        devs = [cm.Device(sample_rate=sr, sfmt=sfmt, channels=[cm.Channel(bin=b) for b in bl]) for bl in self.bin_lists]
+        self.bpc = 2 * cm.BYTES_PER_SAMPLE[sfmt]
+        sr = (hop_bytes // self.bpc) * wave_rate
+        devs = [cm.Device(sample_rate=sr, sfmt=sfmt, fullscale=fullscale,
+                          channels=[cm.Channel(bin=b, afc=4 if d in afc else 0) for b in bl]) for d, bl in enumerate(self.bin_lists)]
+        self.fullscale = devs[0].fullscale
         self.cfg = cm.Config(fft_size=n, wave_rate=wave_rate, devices=devs)
-        assert all(self.cfg.hop(d) * 2 == hop_bytes for d in range(len(devs)))
+        assert all(self.cfg.hop(d) * self.bpc == hop_bytes for d in range(len(devs)))
         self.g0 = np.concatenate([[0], np.cumsum([len(b) for b in self.bin_lists])]).astype(int)
-        self.raws = streams or [make_stream(seed0 + d, n, hop_bytes, sfmt, self.frames(d), self.bin_lists[d][0] if d % 3 else None)
-                                for d in range(len(devs))]
+        self.raws = streams or [make_stream(seed0 + d, n, hop_bytes, sfmt, self.frames(d), self.bin_lists[d][0] if d % 3 else None,
+                                            self.fullscale, rails) for d in range(len(devs))]
 
     def frames(self, d):
         return AGC + self.batches[d] * self.B
@@ -49,21 +54,48 @@ class Group:
     def tables(self):
         return len({tuple(b) for b in self.bin_lists})
 
+    def frame_bytes(self, d, frames):
+        """raw bytes [len(frames), n * bytes per complex sample] of device d's stream frames `frames`."""
+        start = np.asarray(frames, np.int64) * self.hop_bytes
+        return self.raws[d][start[:, None] + np.arange(self.n * self.bpc)[None, :]]
 
-def make_stream(seed, n, hop_bytes, sfmt, frames, tone_bin):
-    """frames * hop_bytes + 2n raw bytes: noise of +-44 codes around mid-scale, plus (tone_bin not None) a carrier of 70 codes
-    on the centre of that bin; a third of the devices get noise alone, where no bin dominates the error bound's scale."""
+
+def make_stream(seed, n, hop_bytes, sfmt, frames, tone_bin, fullscale=None, rails=False):
+    """frames * hop_bytes + one frame of raw bytes.  8-bit: noise of +-44 codes around mid-scale, plus (tone_bin not None) a
+    carrier of 70 codes on the centre of that bin, and with `rails` every 13th sample component at a rail code.  S16: the same
+    shape at 256 times the amplitude, with rails at +-32767 and -32768.  F32: noise at 1e-2 of fullscale, or (tone_bin not
+    None) a carrier at 0.5 of fullscale on that bin, one 100 dB weaker on bin tone_bin + n/4, and noise 140 dB below the
+    carrier.  A third of the devices get noise alone, where no bin dominates the error bound's scale."""
     rng = np.random.default_rng(seed)
-    nbytes = frames * hop_bytes + 2 * n
-    x = rng.integers(-44, 45, nbytes, dtype=np.int16)
-    if tone_bin is not None:
-        t = np.exp(2j * np.pi * tone_bin * np.arange(n) / n + 1j * seed)
+    bps = cm.BYTES_PER_SAMPLE[sfmt]
+    nvals = (frames * hop_bytes) // bps + 2 * n
+    t = np.arange(n)
+
+    def tone(b, amp, phase):
+        z = amp * np.exp(2j * np.pi * b * t / n + 1j * phase)
         one = np.empty(2 * n)
-        one[0::2], one[1::2] = 70 * t.real, 70 * t.imag
-        x += np.resize(np.rint(one).astype(np.int16), nbytes)
+        one[0::2], one[1::2] = z.real, z.imag
+        return np.resize(one, nvals)
+
+    if sfmt == cm.SFMT_F32:
+        if tone_bin is None:
+            x = 1e-2 * fullscale * rng.standard_normal(nvals)
+        else:
+            x = fullscale * (tone(tone_bin, 0.5, seed) + tone(tone_bin + n // 4, 0.5e-5, 2 * seed) + 0.5e-7 * rng.standard_normal(nvals))
+        return x.astype(np.float32).view(np.uint8)
+    x = rng.integers(-44, 45, nvals, dtype=np.int16).astype(np.int64)
+    if tone_bin is not None:
+        x += np.rint(tone(tone_bin, 70, seed)).astype(np.int64)
+    if sfmt == cm.SFMT_S16:
+        x *= 256
+        if rails:
+            x[::13] = rng.choice([32767, -32767, -32768], x[::13].size)
+        return x.astype(np.int16).view(np.uint8)
+    if rails:
+        x[::13] = rng.choice([-128, 127], x[::13].size)
     if sfmt == cm.SFMT_U8:
-        return (x + 128).astype(np.uint8)
-    return x.astype(np.int8).view(np.uint8)
+        return (np.clip(x, -128, 127) + 128).astype(np.uint8)
+    return np.clip(x, -128, 127).astype(np.int8).view(np.uint8)
 
 
 def k1_run(group, fft_mode, nbmax=4, runs=1):
@@ -104,10 +136,10 @@ def check_against_float64(group, win, iq, digits=4, first_batch=0, n_batches=Non
         if nb <= 0:
             continue
         rows = float64_frames(group, d, first_batch * group.B, nb * group.B, rng)
-        start = (AGC + first_batch * group.B + rows) * group.hop_bytes
-        raw = group.raws[d][start[:, None] + np.arange(2 * group.n)[None, :]]
+        raw = group.frame_bytes(d, AGC + first_batch * group.B + rows)
         ref = reference_bins(raw, group.sfmt, group.n, bins)
         cols = slice(group.g0[d], group.g0[d + 1])
+        assert_win_is_magnitude(win[rows, cols], iq[rows, cols])
         scale = np.abs(ref).max()
         err = np.abs(iq[rows, cols] - ref).max() / scale
         assert err < bound, f"device {d} (bins {bins}): X differs from float64 by {err:.3e} of {scale:.4g}, first bad row {rows[np.argmax(np.abs(iq[rows, cols] - ref).max(1))]}"
@@ -115,6 +147,14 @@ def check_against_float64(group, win, iq, digits=4, first_batch=0, n_batches=Non
         assert werr.max() / scale < bound, f"device {d}: |X| differs from float64 by {werr.max() / scale:.3e}"
         worst = max(worst, err)
     return worst
+
+
+def assert_win_is_magnitude(win, iq):
+    """win is the correctly rounded float32 sqrtf(fl(fl(re*re) + fl(im*im))) of the stored iqin, the reference's association
+    (rtl_airband.cpp:484); numpy's float32 square root is correctly rounded too."""
+    re, im = np.real(iq).astype(np.float32), np.imag(iq).astype(np.float32)
+    want = np.sqrt((re * re) + (im * im))
+    assert np.array_equal(win.view(np.uint32), want.view(np.uint32)), f"win differs from |iqin| at {np.argwhere(win != want)[:4].tolist()}"
 
 
 def check_every_row_against_fp32_kernel(group, win, iq, fwin, fiq):
