@@ -361,6 +361,52 @@ ABG_API int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t
  * (0 if that run computed no output).  Waits for it. */
 ABG_API int abg_debug_subband_time(abg_engine* e, float* ms);
 
+/* CTCSS tone meter (not part of the reference surface: the CTCSS gate only works if the operator knows which tone each
+ * transmitter sends, and an SDR program's CTCSS decoder or a scanner would need the dongle to find out).  Per channel and
+ * batch it measures how much of each sub-audible tone of a list is in the audio the channel produced.
+ * B = WAVE_BATCH.  A device's audio batch number a counts the batches it queued for abg_fetch_batch since abg_create,
+ * pushed and injected alike (for a pushed device it is the batch_seq of the other monitors).  y[c][aB + j] = waveout[c][j]
+ * of that batch, exactly as abg_fetch_batch returns it: the audio after the squelch gate, notch, ampfactor and clamp
+ * (reference src/rtl_airband.cpp:584-611).  The tone list f_k, k < K <= ABG_TONE_MAX, applies to the whole engine; by
+ * default it is the reference's 51 standard tones (CTCSS::standard_tones, src/ctcss.cpp:87-89).
+ *     delta_k   = llround(f_k / wave_rate * 2^32) mod 2^32; the tone measured is delta_k * wave_rate / 2^32
+ *     S[c][k]   = sum_{j<B} y[c][aB+j] * exp(-2 pi i ((delta_k * (aB+j)) mod 2^32) / 2^32)     complex float32
+ *     E[c]      = sum_{j<B} y[c][aB+j]^2                                                        float32
+ *     active[c] = number of j with y[c][aB+j] != 0                                              int32
+ * The phase is exact integer arithmetic on the absolute audio index, so the S of consecutive batches add up to the DFT of
+ * the longer window: the reference needs 0.4 s to tell every standard tone apart (src/squelch.cpp:111-115), and 4 batches
+ * (0.5 s) added on the host give that.  A tone of amplitude A at f_k gives |S| ~ A n / 2 over n samples, and its share of
+ * the audio power is 2 |S|^2 / (n E).  Every sum is taken in a fixed order that depends on (B, K) only, so readings are
+ * bitwise reproducible whenever the audio is.  Against the sums in float64 with the exact phase, each component of S is
+ * within (B + 8) * 2^-23 * sum_j |y_j| and E within (B + 1) * 2^-24 * E; active is exact.
+ * Caveats: the meter sees the audio after the gate, so it reads zeros while the squelch is closed; a channel with ctcss
+ * set only opens on its own tone (to find an unknown tone, run the channel without ctcss); a notch set at the tone
+ * removes it.
+ * Computed on the GPU by one extra kernel per run on the K2 stream (stream B), after K2 and the mixers and before the
+ * end-of-run export: while the meter is on its time is part of abg_last_run_times ms4[2] and ms4[3].  With every device
+ * off (the default) nothing is launched, allocated or copied.  Resident runs (abg_run_resident) compute readings but queue
+ * none; batches fed through abg_debug_inject_wavein produce readings like pushed ones. */
+#define ABG_TONE_MAX 64
+/* abg_tone_meter_configure: on = 1 / 0 switches the meter on / off for the device's batches enqueued by later abg_run /
+ * abg_run_resident / abg_debug_inject_wavein calls.  ABG_ERANGE for a bad device, ABG_EINVAL for any other value of on.
+ * Waits for the engine's K2 stream. */
+ABG_API int abg_tone_meter_configure(abg_engine* e, int dev, int on);
+/* Set the engine's tone list for batches of later runs: freqs[n_tones] in Hz, each finite and in (0, wave_rate / 2);
+ * freqs == NULL or n_tones == 0 restores the 51 standard tones.  ABG_EINVAL for n_tones outside [0, ABG_TONE_MAX] or a bad
+ * frequency (the list is then unchanged).  Waits for the engine's K2 stream. */
+ABG_API int abg_tone_meter_set_tones(abg_engine* e, int n_tones, const float* freqs);
+/* Pop the oldest unfetched reading of a device: tones[n_channels][K][2] = S (re, im), energy[n_channels] = E,
+ * active[n_channels] (any may be NULL; tones needs room for K = the tone count it was computed with, at most
+ * ABG_TONE_MAX), batch_seq = a, n_tones = K.  Returns 1 if one was popped, 0 if none is ready, < 0 on error; waits for the
+ * run that computed it.  The queue is lossy exactly like the spectrum's: max_batches_per_run + 2 readings per device, the
+ * oldest overwritten first; the meter never holds a result slot or causes ABG_EOVERFLOW, and readings already queued stay
+ * fetchable, with the K they were computed with, after the meter is switched off or the tone list changed. */
+ABG_API int abg_fetch_tone_meter(abg_engine* e, int dev, float* tones, float* energy, int32_t* active, uint64_t* batch_seq,
+                                 int32_t* n_tones);
+/* Measurement aid: device time of the tone meter kernel of the most recent run, from CUDA events around it on the K2
+ * stream (0 if that run metered nothing).  Waits for it. */
+ABG_API int abg_debug_tone_meter_time(abg_engine* e, float* ms);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

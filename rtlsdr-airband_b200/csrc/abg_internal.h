@@ -256,6 +256,30 @@ struct SbArgs {
 cudaError_t abg_launch_subband(const SbArgs& a, int n_devices, int max_items, int max_hist, cudaStream_t s);
 int abg_subband_chunks(int batch_samples);  // work items per batch of a device
 
+// CTCSS tone meter (tone_meter.cu): see abg_tone_meter_configure in include/airband_b200.h
+#define ABG_TM_COLS 64  // tone-table columns per tile: 32 tones, cos and -sin interleaved
+struct TmCfg {  // per metered device; written by abg_tone_meter_configure
+    float* ring;       // device view of the page-locked result ring [ring_cap][n_channels * (2 * ABG_TONE_MAX + 2)] floats
+    int32_t g0, n_channels;
+    int32_t first;     // index of the device's channel 0 in the metered channel list
+    int32_t ring_cap;
+};
+struct TmRun {  // per metered device; uploaded with every run
+    unsigned long long seq0;  // audio batch number of the run's first batch
+    int32_t n_batches;        // batches of this run (0 = none)
+    int32_t ring_pos0;        // ring entry of the run's first batch; < 0: resident run, the ring is left alone
+};
+struct TmArgs {
+    const TmCfg* cfg;         // [metered devices]
+    const TmRun* run;
+    const int32_t* chan_dev;  // [n_chan] metered channel -> index into cfg / run
+    const float* table;       // [wave_batch][n_cols]: cos, -sin of (delta_k * j mod 2^32) 2 pi / 2^32, zero columns past 2K
+    const float* wout;        // [Gp][P] the run's audio, batch b of channel g at g * P + b * wave_batch
+    int P, wave_batch, K, n_cols, n_chan;
+    uint32_t delta[ABG_TONE_MAX];
+};
+cudaError_t abg_launch_tone_meter(const TmArgs& a, int max_batches, cudaStream_t s);
+
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B
     int lanes_per_warp;       // channels handled by one warp of K2: 1, 2, 4, 8, 16 or 32

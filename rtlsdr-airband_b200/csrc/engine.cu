@@ -168,15 +168,15 @@ struct DevBuf {
     }
 };
 
-// Result queue of one device's batch monitor (band spectrum, carrier meter, input level meter, sub-band output).  The
-// monitor's kernel writes the result of every batch straight into a page-locked, mapped ring of `cap` =
+// Result queue of one device's batch monitor (band spectrum, carrier meter, input level meter, sub-band output, tone
+// meter).  The monitor's kernel writes the result of every batch straight into a page-locked, mapped ring of `cap` =
 // max_batches_per_run + 2 entries; the host keeps the unfetched entries, oldest first.  Lossy by design: queueing a run
 // drops the oldest unfetched entries beyond the ring's size (gaps show in their batch_seq), so a monitor never holds a
 // result slot or causes ABG_EOVERFLOW.
 struct MonitorQueue {
     struct Entry {
         int pos;      // ring entry
-        int32_t aux;  // monitor-specific: frames averaged (spectrum), decimation (sub-band output), 0 otherwise
+        int32_t aux;  // monitor-specific: frames averaged (spectrum), decimation (sub-band output), tones (tone meter), 0 otherwise
         uint64_t seq, run;
     };
     unsigned char* ring = nullptr;  // [cap][entry_bytes]; allocated when the monitor is first switched on, kept until abg_destroy
@@ -258,6 +258,7 @@ struct Device {
     float2* spec = nullptr;  // [nbmax][N] when has_afc
     std::deque<std::pair<int, int>> ready;  // (slot, batch-in-run)
     uint64_t batch_seq = 0;  // batches of the pushed stream enqueued since abg_create
+    uint64_t audio_seq = 0;  // batches queued for abg_fetch_batch since abg_create, pushed and injected
     // band spectrum monitor (abg_spectrum_configure); nothing is allocated until it is first switched on
     int spec_stride = 0, spec_n_sel = 0, spec_chunks = 0;
     void* spec_work = nullptr;   // device: chunk sums float[nbmax][spec_chunks][N], then the batch counters int32[nbmax]
@@ -282,6 +283,9 @@ struct Device {
     } sb[ABG_SUBBAND_MAX];
     int sb_hist = 0;                 // L_max - 1 over the outputs switched on: samples compaction keeps before `consumed`
     size_t dropped = 0;              // stream bytes compaction has dropped: raw[cur][0] is byte `dropped` of the stream
+    // CTCSS tone meter (abg_tone_meter_configure); nothing is allocated until it is first switched on
+    bool tm_on = false;
+    MonitorQueue tm_q;               // S float[C][K][2], E float[C], active int32[C] per entry (room for ABG_TONE_MAX), Entry.aux = K
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -416,11 +420,19 @@ struct abg_engine {
     cudaEvent_t tl[TL_RUNS][5] = {};
     bool tev_valid = false;
     std::vector<int32_t> h_bins;
-    // batch monitors, launched in this order on stream A after K1
+    // batch monitors: the first four are launched in this order on stream A after K1, the tone meter on stream B after K2
     MonitorLaunch<SpecCfg, SpecRun> spectrum{"spectrum", true};
     MonitorLaunch<CarCfg, CarRun> carrier{"carrier meter", false};
     MonitorLaunch<InmCfg, InmRun> input_meter{"input meter", true};
     MonitorLaunch<SbCfg, SbRun> subband{"sub-band", true};
+    MonitorLaunch<TmCfg, TmRun> tone_meter{"tone meter", false};
+    // tone meter tables: the engine-wide tone list and, once the meter is first switched on, its [B][tm_cols] table
+    std::vector<float> tm_freqs{std::begin(kStandardTones), std::end(kStandardTones)};
+    std::vector<uint32_t> tm_delta;
+    DevBuf<float> tm_table;
+    int tm_cols = 0;
+    DevBuf<int32_t> tm_chan_dev;  // metered channel -> index into tone_meter.devs
+    int tm_n_chan = 0;
     int sb_max_hist = 0;  // largest Device::sb_hist of subband.devs
     // after the last monitor that read raw[] in the latest run of each parity that launched one; created when the first
     // such monitor is switched on
@@ -475,22 +487,22 @@ int monitor_publish(abg_engine* e, MonitorLaunch<Cfg, Run>& m, const std::vector
     return ABG_OK;
 }
 
-// One run of a monitor on stream A, after its h_run records are filled: their upload, then `kernel(n_devices,
-// max_items, stream)` between the timing events, then ev_raw if it reads raw[].  Nothing when max_items is 0.
+// One run of a monitor on stream st (A after K1, or B after K2), after its h_run records are filled: their upload, then
+// `kernel(n_devices, max_items, stream)` between the timing events, then ev_raw if it reads raw[].  Nothing when max_items
+// is 0.
 template <typename Cfg, typename Run, typename Kernel>
-int monitor_launch(abg_engine* e, MonitorLaunch<Cfg, Run>& m, int max_items, Kernel&& kernel) {
+int monitor_launch(abg_engine* e, MonitorLaunch<Cfg, Run>& m, int max_items, cudaStream_t st, Kernel&& kernel) {
     if (max_items <= 0) return ABG_OK;
-    cudaStream_t sa = e->stream;
     const int t = (int)(e->run_index % TL_RUNS);
-    const int nl = upload_small(m.run.p, m.h_run.data(), sizeof(Run) * m.devs.size(), sa);
+    const int nl = upload_small(m.run.p, m.h_run.data(), sizeof(Run) * m.devs.size(), st);
     if (nl < 0) return fail(ABG_ECUDA, "%s parameter upload failed: %s", m.name, cudaGetErrorString(cudaGetLastError()));
     e->launches += (uint64_t)nl;
-    CU(cudaEventRecord(m.tl[t][0], sa));
-    const cudaError_t er = kernel((int)m.devs.size(), max_items, sa);
+    CU(cudaEventRecord(m.tl[t][0], st));
+    const cudaError_t er = kernel((int)m.devs.size(), max_items, st);
     if (er != cudaSuccess) return fail(ABG_ECUDA, "%s launch failed: %s", m.name, cudaGetErrorString(er));
     e->launches++;
-    CU(cudaEventRecord(m.tl[t][1], sa));
-    if (m.reads_raw) CU(cudaEventRecord(e->ev_raw[e->run_index & 1], sa));
+    CU(cudaEventRecord(m.tl[t][1], st));
+    if (m.reads_raw) CU(cudaEventRecord(e->ev_raw[e->run_index & 1], st));
     m.ran[t] = true;
     return ABG_OK;
 }
@@ -545,6 +557,7 @@ void engine_free(abg_engine* e) {
         d.spec_q.release();
         d.car_q.release();
         d.inm_q.release();
+        d.tm_q.release();
         for (auto& so : d.sb) {
             if (so.coef) cudaFree(so.coef);
             so.q.release();
@@ -554,6 +567,9 @@ void engine_free(abg_engine* e) {
     monitor_free(e->carrier);
     monitor_free(e->input_meter);
     monitor_free(e->subband);
+    monitor_free(e->tone_meter);
+    e->tm_table.free();
+    e->tm_chan_dev.free();
     for (auto& g : e->groups) {
         g.wsc.free();
         g.tc_btab.free(); g.tc_sq.free(); g.tc_tab_of_dev.free();
@@ -1082,7 +1098,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     // ---- batch monitors (stream A after K1 in this order: the spectrum, the carrier meter, the input meter, the sub-band
     // outputs; K2 does not wait for them past ev_k1).  Injected batches have no frames and launch none. ----
     const int t = (int)(ri % TL_RUNS);
-    e->spectrum.ran[t] = e->carrier.ran[t] = e->input_meter.ran[t] = e->subband.ran[t] = false;
+    e->spectrum.ran[t] = e->carrier.ran[t] = e->input_meter.ran[t] = e->subband.ran[t] = e->tone_meter.ran[t] = false;
     if (!skip_k1) {
         int max_items = 0;
         for (size_t m = 0; m < e->spectrum.devs.size(); m++) {
@@ -1095,7 +1111,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             r.ring_pos0 = queue_outputs && n > 0 ? d.spec_q.queue(n, d.batch_seq, ri, d.spec_n_sel) : -1;
             max_items = std::max(max_items, n * d.spec_chunks);
         }
-        int rc = monitor_launch(e, e->spectrum, max_items, [&](int n_devices, int items, cudaStream_t s) {
+        int rc = monitor_launch(e, e->spectrum, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
             SpecArgs A{};
             A.cfg = e->spectrum.cfg.p; A.run = e->spectrum.run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
             return abg_launch_spectrum(N, A, n_devices, items, s);
@@ -1111,7 +1127,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             r.ring_pos0 = queue_outputs && n > 0 ? d.car_q.queue(n, d.batch_seq, ri, 0) : -1;
             max_items = std::max(max_items, n * abg_carrier_items(d.C));
         }
-        rc = monitor_launch(e, e->carrier, max_items, [&](int n_devices, int items, cudaStream_t s) {
+        rc = monitor_launch(e, e->carrier, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
             CarArgs A{};
             A.cfg = e->carrier.cfg.p; A.run = e->carrier.run.p; A.iqin = e->iqin[cur].p; A.Gp = e->Gp; A.wave_batch = B;
             return abg_launch_carrier(A, n_devices, items, s);
@@ -1128,7 +1144,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             r.ring_pos0 = queue_outputs && n > 0 ? d.inm_q.queue(n, d.batch_seq, ri, 0) : -1;
             max_items = std::max(max_items, n * d.inm_chunks);
         }
-        rc = monitor_launch(e, e->input_meter, max_items, [&](int n_devices, int items, cudaStream_t s) {
+        rc = monitor_launch(e, e->input_meter, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
             InmArgs A{};
             A.cfg = e->input_meter.cfg.p; A.run = e->input_meter.run.p; A.wave_batch = B;
             return abg_launch_input_meter(A, n_devices, items, s);
@@ -1156,7 +1172,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             }
             max_items = std::max(max_items, n * abg_subband_chunks(B * d.hop));
         }
-        rc = monitor_launch(e, e->subband, max_items, [&](int n_devices, int items, cudaStream_t s) {
+        rc = monitor_launch(e, e->subband, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
             SbArgs A{};
             A.cfg = e->subband.cfg.p; A.run = e->subband.run.p;
             return abg_launch_subband(A, n_devices, items, e->sb_max_hist, s);
@@ -1194,6 +1210,29 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
         if (er != cudaSuccess) return fail(ABG_ECUDA, "mixer launch failed: %s", cudaGetErrorString(er));
         e->launches++;
     }
+    // ---- tone meter (stream B after K2 and the mixers, pushed and injected batches alike): it reads wout[0, nb*B) before
+    // the tail copy below overwrites [0, AGC_EXTRA), and the next run's K2 queues behind it on this stream ----
+    {
+        const int K = (int)e->tm_freqs.size();
+        int max_items = 0;
+        for (size_t m = 0; m < e->tone_meter.devs.size(); m++) {
+            Device& d = e->dev[e->tone_meter.devs[m]];
+            const int n = nb[e->tone_meter.devs[m]];
+            TmRun& r = e->tone_meter.h_run[m];
+            r.seq0 = d.audio_seq;
+            r.n_batches = n;
+            r.ring_pos0 = queue_outputs && n > 0 ? d.tm_q.queue(n, d.audio_seq, ri, K) : -1;
+            max_items = std::max(max_items, n);
+        }
+        const int rc = monitor_launch(e, e->tone_meter, max_items, sb, [&](int, int items, cudaStream_t s) {
+            TmArgs A{};
+            A.cfg = e->tone_meter.cfg.p; A.run = e->tone_meter.run.p; A.chan_dev = e->tm_chan_dev.p; A.table = e->tm_table.p;
+            A.wout = e->wout.p; A.P = e->P; A.wave_batch = B; A.K = K; A.n_cols = e->tm_cols; A.n_chan = e->tm_n_chan;
+            for (int k = 0; k < K; k++) A.delta[k] = e->tm_delta[k];
+            return abg_launch_tone_meter(A, items, s);
+        });
+        if (rc != ABG_OK) return rc;
+    }
     // ---- results: the end-of-run kernel writes them straight into the pinned slot, then does the consumer's tail copy ----
     K2Export X{};
     if (queue_outputs) {
@@ -1228,6 +1267,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     for (size_t i = 0; i < e->dev.size(); i++) {
         if (nb[i] <= 0) continue;
         Device& d = e->dev[i];
+        if (!resident) d.audio_seq += (uint64_t)nb[i];
         if (skip_k1) {
             // nothing was consumed from the raw stream
         } else if (resident) {
@@ -1739,6 +1779,113 @@ int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t* batch_
 }
 
 int abg_debug_subband_time(abg_engine* e, float* ms) { return monitor_time(e, e->subband, ms, __func__); }
+
+// ---- CTCSS tone meter (definition in airband_b200.h) -------------------------------------------------------------------
+// The tone table of the current list: T[j][2k] = cos, T[j][2k+1] = -sin of 2 pi (delta_k j mod 2^32) / 2^32, built in double
+// and rounded once to float32; columns 2K .. tm_cols are zero.  The caller has waited for stream B.
+static int tone_meter_table(abg_engine* e) {
+    const int K = (int)e->tm_freqs.size(), B = e->B;
+    const int cols = (2 * K + ABG_TM_COLS - 1) / ABG_TM_COLS * ABG_TM_COLS;
+    e->tm_delta.resize(K);
+    for (int k = 0; k < K; k++)
+        e->tm_delta[k] = (uint32_t)(unsigned long long)llround((double)e->tm_freqs[k] / e->W * 4294967296.0);
+    std::vector<float> t((size_t)B * cols, 0.0f);
+    for (int j = 0; j < B; j++)
+        for (int k = 0; k < K; k++) {
+            const double turns = (double)(int32_t)(e->tm_delta[k] * (uint32_t)j) * 0x1p-32;  // exact, in [-1/2, 1/2)
+            t[(size_t)j * cols + 2 * k] = (float)cos(2.0 * M_PI * turns);
+            t[(size_t)j * cols + 2 * k + 1] = (float)-sin(2.0 * M_PI * turns);
+        }
+    if (cols != e->tm_cols) {
+        e->tm_table.free();
+        e->tm_cols = 0;
+        if (e->tm_table.alloc(t.size())) {
+            e->tm_table.p = nullptr;
+            return fail(ABG_ENOMEM, "Out of device memory for the tone meter table");
+        }
+        e->tm_cols = cols;
+    }
+    CU(cudaMemcpy(e->tm_table.p, t.data(), sizeof(float) * t.size(), cudaMemcpyHostToDevice));
+    return ABG_OK;
+}
+
+int abg_tone_meter_configure(abg_engine* e, int dev, int on) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_tone_meter_configure: device %d out of range", dev);
+    if (on != 0 && on != 1) return fail(ABG_EINVAL, "abg_tone_meter_configure: on = %d is neither 0 nor 1", on);
+    Device& d = e->dev[dev];
+    if ((on == 1) == d.tm_on) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream_b));  // an enqueued meter kernel may still read the device tables
+    if (on) {
+        if (monitor_on(e, e->tone_meter) != ABG_OK) return ABG_ECUDA;
+        if (!d.tm_q.alloc(e->nbmax + 2, sizeof(float) * (2 * ABG_TONE_MAX + 2) * (size_t)std::max(d.C, 1)))
+            return fail(ABG_ENOMEM, "Out of page-locked host memory for the tone meter ring");
+        if (!e->tm_table.p) {
+            const int rc = tone_meter_table(e);
+            if (rc != ABG_OK) return rc;
+        }
+    }
+    d.tm_on = on == 1;
+    // rebuild the launch's device list, its static table and the channel map
+    std::vector<int> devs;
+    std::vector<TmCfg> cfgs;
+    std::vector<int32_t> chan_dev;
+    for (int i = 0; i < (int)e->dev.size(); i++) {
+        const Device& x = e->dev[i];
+        if (!x.tm_on) continue;
+        TmCfg c{};
+        CU(cudaHostGetDevicePointer((void**)&c.ring, x.tm_q.ring, 0));
+        c.g0 = x.g0; c.n_channels = x.C; c.first = (int32_t)chan_dev.size(); c.ring_cap = x.tm_q.cap;
+        chan_dev.insert(chan_dev.end(), x.C, (int32_t)devs.size());
+        devs.push_back(i);
+        cfgs.push_back(c);
+    }
+    e->tm_chan_dev.free();
+    e->tm_n_chan = 0;
+    if (!chan_dev.empty()) {
+        if (e->tm_chan_dev.alloc(chan_dev.size())) {
+            e->tm_chan_dev.p = nullptr;
+            return fail(ABG_ENOMEM, "Out of device memory for the tone meter tables");
+        }
+        CU(cudaMemcpy(e->tm_chan_dev.p, chan_dev.data(), sizeof(int32_t) * chan_dev.size(), cudaMemcpyHostToDevice));
+        e->tm_n_chan = (int)chan_dev.size();
+    }
+    return monitor_publish(e, e->tone_meter, devs, cfgs);
+}
+
+int abg_tone_meter_set_tones(abg_engine* e, int n_tones, const float* freqs) {
+    if (n_tones < 0 || n_tones > ABG_TONE_MAX)
+        return fail(ABG_EINVAL, "abg_tone_meter_set_tones: %d tones outside [0, %d]", n_tones, ABG_TONE_MAX);
+    std::vector<float> list(std::begin(kStandardTones), std::end(kStandardTones));
+    if (freqs && n_tones > 0) {
+        list.assign(freqs, freqs + n_tones);
+        for (int k = 0; k < n_tones; k++)
+            if (!std::isfinite(freqs[k]) || !(freqs[k] > 0.0f) || !((double)freqs[k] < e->W / 2.0))
+                return fail(ABG_EINVAL, "abg_tone_meter_set_tones: tone %d (%g Hz) outside (0, %d) Hz", k, (double)freqs[k], e->W / 2);
+    }
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream_b));  // an enqueued meter kernel may still read the table
+    e->tm_freqs = list;
+    return e->tm_table.p ? tone_meter_table(e) : ABG_OK;
+}
+
+int abg_fetch_tone_meter(abg_engine* e, int dev, float* tones, float* energy, int32_t* active, uint64_t* batch_seq, int32_t* n_tones) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_tone_meter: device %d out of range", dev);
+    const unsigned char* src = nullptr;
+    MonitorQueue::Entry r{};
+    const size_t C = (size_t)e->dev[dev].C;
+    const int rc = monitor_pop(e, e->dev[dev].tm_q, e->tone_meter, &src, &r);
+    if (rc <= 0) return rc;
+    const size_t K = (size_t)r.aux;
+    if (tones) memcpy(tones, src, sizeof(float) * 2 * K * C);
+    if (energy) memcpy(energy, src + sizeof(float) * 2 * K * C, sizeof(float) * C);
+    if (active) memcpy(active, src + sizeof(float) * (2 * K + 1) * C, sizeof(int32_t) * C);
+    if (batch_seq) *batch_seq = r.seq;
+    if (n_tones) *n_tones = r.aux;
+    return 1;
+}
+
+int abg_debug_tone_meter_time(abg_engine* e, float* ms) { return monitor_time(e, e->tone_meter, ms, __func__); }
 
 // ---- scan mode -------------------------------------------------------------------------------------------------------
 static ScanView scan_view(abg_engine* e) {

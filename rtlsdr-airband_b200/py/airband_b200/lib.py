@@ -27,10 +27,17 @@ SYMBOLS = [
     "abg_carrier_configure", "abg_fetch_carrier", "abg_debug_carrier_time",
     "abg_input_meter_configure", "abg_fetch_input_levels", "abg_debug_input_meter_time",
     "abg_subband_configure", "abg_fetch_subband", "abg_debug_subband_time",
+    "abg_tone_meter_configure", "abg_tone_meter_set_tones", "abg_fetch_tone_meter", "abg_debug_tone_meter_time",
 ]
 
 SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
 SUBBAND_MAX_COEFFS = 4096  # ABG_SUBBAND_MAX_COEFFS
+TONE_MAX = 64              # ABG_TONE_MAX: tones in the tone meter's list
+# the tone meter's default list: the reference's standard CTCSS tones (CTCSS::standard_tones, src/ctcss.cpp:87-89)
+STANDARD_TONES = (67.0, 69.3, 71.9, 74.4, 77.0, 79.7, 82.5, 85.4, 88.5, 91.5, 94.8, 97.4, 100.0, 103.5, 107.2, 110.9, 114.8,
+                  118.8, 123.0, 127.3, 131.8, 136.5, 141.3, 146.2, 150.0, 151.4, 156.7, 159.8, 162.2, 165.5, 167.9, 171.3,
+                  173.8, 177.3, 179.9, 183.5, 186.2, 189.9, 192.8, 196.6, 199.5, 203.5, 206.5, 210.7, 218.1, 225.7, 229.1,
+                  233.6, 241.8, 250.3, 254.1)
 
 
 class COptions(C.Structure):
@@ -131,6 +138,11 @@ def load():
     L.abg_fetch_subband.restype = i
     L.abg_fetch_subband.argtypes = [vp, i, i, vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
     L.abg_debug_subband_time.restype, L.abg_debug_subband_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_tone_meter_configure.restype, L.abg_tone_meter_configure.argtypes = i, [vp, i, i]
+    L.abg_tone_meter_set_tones.restype, L.abg_tone_meter_set_tones.argtypes = i, [vp, i, vp]
+    L.abg_fetch_tone_meter.restype = i
+    L.abg_fetch_tone_meter.argtypes = [vp, i, vp, vp, vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
+    L.abg_debug_tone_meter_time.restype, L.abg_debug_tone_meter_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -403,6 +415,36 @@ class Engine:
         """ms of the sub-band kernel in the most recent run (CUDA events on the K1 stream); 0 if it computed nothing."""
         return self._kernel_time(self.L.abg_debug_subband_time)
 
+    # ---- CTCSS tone meter -----------------------------------------------------------------------------------------
+    def tone_meter_configure(self, dev: int, on: bool) -> None:
+        """DFT of every channel's audio at each tone of the engine's list, its energy and its non-zero samples, per batch
+        (off by default); applies to batches enqueued by later runs, injected ones included.  `ctcss_identify` names the
+        tone."""
+        self._chk(self.L.abg_tone_meter_configure(self.h, dev, int(on)))
+
+    def tone_meter_set_tones(self, freqs=None) -> None:
+        """The engine's tone list (at most TONE_MAX tones, each in (0, wave_rate / 2) Hz) for batches of later runs; None or
+        an empty list restores STANDARD_TONES."""
+        f = None if freqs is None or len(freqs) == 0 else np.ascontiguousarray(freqs, dtype=np.float32)
+        self._chk(self.L.abg_tone_meter_set_tones(self.h, 0 if f is None else f.size, _ptr(f)))
+
+    def fetch_tone_meter(self, dev: int) -> Optional[Tuple[np.ndarray, np.ndarray, np.ndarray, int]]:
+        """Oldest unfetched reading of a device: (S complex64[C, K], E float32[C], active int32[C], batch_seq), or None.
+        K is the tone count the reading was computed with.  Lossy: at most max_batches_per_run + 2 are kept per device."""
+        Cn = len(self.cfg.devices[dev].channels) if 0 <= dev < len(self.cfg.devices) else 0  # (a bad index: the C call reports it)
+        tones = np.empty(2 * TONE_MAX * Cn, np.float32)
+        energy = np.empty(Cn, np.float32)
+        active = np.empty(Cn, np.int32)
+        seq, k = C.c_uint64(0), C.c_int32(0)
+        if not self._chk(self.L.abg_fetch_tone_meter(self.h, dev, _ptr(tones), _ptr(energy), _ptr(active), C.byref(seq), C.byref(k))):
+            return None
+        K = int(k.value)
+        return tones[:2 * K * Cn].view(np.complex64).reshape(Cn, K).copy(), energy, active, int(seq.value)
+
+    def tone_meter_time(self) -> float:
+        """ms of the tone meter kernel in the most recent run (CUDA events on the K2 stream); 0 if it metered nothing."""
+        return self._kernel_time(self.L.abg_debug_tone_meter_time)
+
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
         """mixers[m] = [(dev, chan, ampfactor, balance), ...]"""
@@ -507,6 +549,54 @@ def subband_frequency(offset_hz: float, sample_rate: float) -> float:
     if delta >= 1 << 31:
         delta -= 1 << 32
     return delta * float(sample_rate) / 4294967296.0
+
+
+def tone_meter_frequency(f: float, wave_rate: float) -> float:
+    """The frequency the tone meter measures for a listed tone f: delta * wave_rate / 2^32 with
+    delta = llround(f / wave_rate * 2^32) (f in (0, wave_rate / 2))."""
+    x = float(np.float32(f)) / float(wave_rate) * 4294967296.0
+    return int(np.floor(x + 0.5)) * float(wave_rate) / 4294967296.0
+
+
+def tone_powers(readings) -> np.ndarray:
+    """Power share of each tone over consecutive tone meter readings of one device (Engine.fetch_tone_meter tuples, oldest
+    first): with S, E and n = active summed over the readings, 2 |S|^2 / (n E), float64[C, K].  Adding S gives the DFT of
+    the whole window, since the meter's phase is that of the absolute audio index.  n counts the samples with audio, so a
+    squelch that was closed for part of the window does not dilute the share; a channel without audio reads 0.  A pure
+    tone reads about 1.  Raises ValueError on a gap in batch_seq or a change of the tone count."""
+    readings = list(readings)
+    if not readings:
+        raise ValueError("tone_powers: no readings")
+    S = np.zeros(readings[0][0].shape, np.complex128)
+    E = np.zeros(readings[0][1].shape, np.float64)
+    n = np.zeros(readings[0][2].shape, np.float64)
+    for i, (s, e, a, seq) in enumerate(readings):
+        if s.shape != S.shape:
+            raise ValueError(f"tone_powers: reading {i} has {s.shape[-1]} tones, the first has {S.shape[-1]}")
+        if i and seq != readings[i - 1][3] + 1:
+            raise ValueError(f"tone_powers: gap in batch_seq: {readings[i - 1][3]} then {seq}")
+        S += s
+        E += e
+        n += a
+    den = n * E
+    with np.errstate(divide="ignore", invalid="ignore"):
+        share = np.where(den[:, None] > 0, 2.0 * np.abs(S) ** 2 / den[:, None], 0.0)
+    return share
+
+
+def ctcss_identify(readings, min_share: float = 0.005, tones: Optional[Sequence[float]] = None):
+    """The CTCSS tone of each channel from consecutive tone meter readings (see tone_powers; 4 batches, 0.5 s, tell every
+    standard tone apart): per channel (tone_hz, share) of the strongest tone, or None when its share is below min_share.
+    tones: the list the readings were computed with (default STANDARD_TONES)."""
+    share = tone_powers(readings)
+    tones = STANDARD_TONES if tones is None else tuple(tones)
+    if len(tones) != share.shape[1]:
+        raise ValueError(f"ctcss_identify: {len(tones)} tones given, the readings have {share.shape[1]}")
+    out = []
+    for row in share:
+        k = int(np.argmax(row))
+        out.append((float(tones[k]), float(row[k])) if row[k] >= min_share else None)
+    return out
 
 
 def subband_lowpass(n_coeffs: int, cutoff_hz: float, sample_rate: float, atten_db: float = 60.0) -> np.ndarray:

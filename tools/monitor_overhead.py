@@ -2,7 +2,7 @@
 process, plus the monitor kernel's own CUDA-event time and K1 / K2.  The card name and power limit are read in the same
 call.
 
-    python tools/monitor_overhead.py --monitor {spectrum,carrier,input_meter,subband} [--workloads cfg2,cfg5] [--runs 40]
+    python tools/monitor_overhead.py --monitor {spectrum,carrier,input_meter,subband,tone_meter} [--workloads cfg2,cfg5] [--runs 40]
                                      [--reps 3] [--out DIR]
 
 Legs:
@@ -11,6 +11,8 @@ Legs:
   input_meter  off, on for every device
   subband      no output, one and four outputs per device (decimation 32, 255 coefficients).  Resident runs compute every
                output but write none to the host rings, so these times leave out the outputs' transfer to host memory.
+  tone_meter   off, on for every device with the 51 standard tones.  As for the sub-band outputs, resident runs leave out
+               the readings' transfer to host memory.
 
 Prints one JSON line per workload (and writes it to DIR/<monitor>_overhead.jsonl with --out).  It uses only public
 lib.Engine methods, so ABG_LIB_PATH can point it at another build of the library."""
@@ -69,6 +71,14 @@ MONITORS = {
         extra=lambda cfg: {"decim": DECIM, "n_coeffs": NTAPS, "raw_bytes_read_per_run": raw_bytes_per_run(cfg),
                            "outputs_per_run_per_output": sum(NB * -(-(cfg.wave_batch * cfg.hop(d)) // DECIM)
                                                              for d in range(len(cfg.devices)))}),
+    "tone_meter": dict(
+        legs=lambda cfg: {"off": False, "on": True},
+        configure=lambda e, cfg, d, on: e.tone_meter_configure(d, on),
+        time="tone_meter_time", time_key="tone_meter_ms",
+        extra=lambda cfg: {"n_tones": len(lib.STANDARD_TONES),
+                           "wout_bytes_read_per_run": NB * cfg.wave_batch * sum(len(d.channels) for d in cfg.devices) * 4,
+                           "gemm_flop_per_run": 2 * NB * sum(len(d.channels) for d in cfg.devices) * cfg.wave_batch
+                           * 2 * len(lib.STANDARD_TONES)}),
 }
 
 
