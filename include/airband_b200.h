@@ -407,6 +407,66 @@ ABG_API int abg_fetch_tone_meter(abg_engine* e, int dev, float* tones, float* en
  * stream (0 if that run metered nothing).  Waits for it. */
 ABG_API int abg_debug_tone_meter_time(abg_engine* e, float* ms);
 
+/* Band activity detector (not part of the reference surface: it answers what is transmitting in the band that no channel
+ * listens to, and when, while the engine holds the SDR; the band spectrum averages a whole batch, so a short burst sinks
+ * into its average).  It reports every burst above a per-bin threshold at the resolution of single frames.
+ * A device with the detector on has a frame stride s >= 1, a hang 0 <= h < n, a minimum span m >= 1 (h and m in selected
+ * frames) and a threshold thr[k] > 0 for each bin k < fft_size, on the scale of the band spectrum's P[k] (|X|^2).
+ *   Frames: batch b (numbered as for the band spectrum) covers f = AGC_EXTRA + b*B + j, j in [0, B), B = WAVE_BATCH.  The
+ *     frames with j % s == 0 are selected, numbered i = j / s in [0, n), n = ceil(B / s); the absolute selected index is
+ *     q = b*n + i.
+ *   Power: p_f[k] = fmaf(re, re, im*im) of X_f[k], the same unnormalised DFT of the converted, windowed frame as the band
+ *     spectrum's, in the same float32 expression.  Frame f is active in bin k iff p_f[k] > thr[k].
+ *   Burst (independent of batches): a maximal set of active selected frames of one bin in which consecutive members are
+ *     at most h + 1 apart in q; it is reported iff q_last - q_first + 1 >= m.  Fields: bin, first_frame and last_frame (f
+ *     of its first and last member), n_active (members), peak = max p, sum = sum of p over its members.
+ *   Pieces: per batch the detector emits the same grouping restricted to the batch's selected frames, with the flags
+ *     ABG_BURST_OPEN_START iff its first i <= h and ABG_BURST_OPEN_END iff its last i >= n - 1 - h.  A piece with neither
+ *     flag and a span < m can never grow and is dropped; every other piece is emitted.  sum is added in frame order in
+ *     float32, so pieces are bitwise reproducible (for every max_batches_per_run, push pattern, fft_mode and set of other
+ *     monitors).
+ *   Merging: a piece with OPEN_END in batch b and one with OPEN_START in batch b + 1, in the same bin, join iff their gap
+ *     in q is <= h + 1; the m filter is applied after joining.  Merging the pieces of consecutive batches this way gives
+ *     exactly the bursts of the definition above: because h < n, a gap that spans a whole batch is longer than h + 1, so
+ *     no join reaches past the next batch.
+ * Capacity: a reading stores at most ABG_ACTIVITY_MAX_RECORDS pieces and counts all of them (n_total, after the drop
+ * above).  When n_total exceeds the capacity the reading is truncated and which pieces are stored is unspecified;
+ * otherwise abg_fetch_activity returns them all, sorted by (bin, first_frame) on the host.
+ * Computed on the GPU by one extra kernel per run on the K1 stream, after K1 and the other monitors of that stream (the
+ * sub-band outputs last); it re-reads the device's raw bytes, K2 does not wait for it.  With every device off (the default)
+ * nothing is launched, allocated or copied.  Resident runs (abg_run_resident) compute pieces but queue none; batches fed
+ * through abg_debug_inject_wavein have no frames and produce none. */
+#define ABG_ACTIVITY_MAX_RECORDS 4096
+enum { ABG_BURST_OPEN_START = 1, ABG_BURST_OPEN_END = 2 };
+typedef struct abg_burst {
+    int32_t bin;              /* natural bin order, 0 .. fft_size-1 */
+    int32_t flags;            /* ABG_BURST_OPEN_START | ABG_BURST_OPEN_END */
+    uint64_t first_frame;     /* absolute frame number f of the first active frame */
+    uint64_t last_frame;      /* ... of the last */
+    int32_t n_active;         /* active selected frames */
+    float peak;               /* max p */
+    float sum;                /* sum of p, in frame order, float32 */
+    int32_t reserved;         /* 0; keeps the size at 40 bytes */
+} abg_burst;
+/* abg_activity_configure: stride = 0 switches the detector off; otherwise it is (re)configured with hang, min_span and
+ * thr[fft_size], for batches enqueued by later abg_run / abg_run_resident calls.  ABG_ERANGE for a bad device; ABG_EINVAL
+ * for a negative argument, and when stride > 0 for a null thr, a threshold that is not finite or is <= 0, stride >
+ * WAVE_BATCH, hang >= ceil(WAVE_BATCH / stride) or min_span < 1.  Waits for the engine's K1 stream. */
+ABG_API int abg_activity_configure(abg_engine* e, int dev, int stride, int hang, int min_span, const float* thr);
+/* Pop the oldest unfetched reading of a device: the first min(n_stored, cap) of its stored pieces, sorted by (bin,
+ * first_frame), into out[cap] (may be NULL with cap = 0); n_stored = pieces the reading stored (min(n_total,
+ * ABG_ACTIVITY_MAX_RECORDS)); n_total = pieces it found (n_total > n_stored: truncated); batch_seq as for
+ * abg_fetch_spectrum; settings3 = {stride, hang, min_span} it was computed with, so that a caller can refuse to stitch
+ * across a change.  Any output pointer may be NULL.  Returns 1 if one was popped, 0 if none is ready, < 0 on error
+ * (ABG_EINVAL for cap < 0); waits for the run that computed it.  The queue is lossy exactly like the spectrum's:
+ * max_batches_per_run + 2 readings per device, the oldest overwritten first; the detector never holds a result slot or
+ * causes ABG_EOVERFLOW, and readings already queued stay fetchable after it is switched off or reconfigured. */
+ABG_API int abg_fetch_activity(abg_engine* e, int dev, abg_burst* out, int cap, int32_t* n_stored, int32_t* n_total,
+                               uint64_t* batch_seq, int32_t* settings3);
+/* Measurement aid: device time of the detector kernel of the most recent run, from CUDA events around it on the K1 stream
+ * (0 if that run detected nothing).  Waits for it. */
+ABG_API int abg_debug_activity_time(abg_engine* e, float* ms);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

@@ -280,6 +280,30 @@ struct TmArgs {
 };
 cudaError_t abg_launch_tone_meter(const TmArgs& a, int max_batches, cudaStream_t s);
 
+// band activity detector (activity.cu): see abg_activity_configure in include/airband_b200.h
+#define ABG_ACT_HEAD_BYTES 16  // ring entry head: int32 {n_total, stride, hang, min_span}, then abg_burst[ABG_ACTIVITY_MAX_RECORDS]
+struct ActCfg {  // per device with the detector on; written by abg_activity_configure
+    const float* wsc;        // the device's K1 window table (window * 1/full-scale)
+    const float* thr;        // [N] per-bin thresholds
+    unsigned char* ring;     // device view of the page-locked result ring [ring_cap][entry_bytes]
+    int32_t hop_bytes, sfmt, stride, n_sel, hang, min_span, ring_cap, entry_bytes;
+};
+struct ActRun {  // per device with the detector on; uploaded with every run
+    const unsigned char* raw;
+    unsigned long long first_byte;   // first byte of frame j = 0 of the run's first batch
+    unsigned long long first_frame;  // absolute frame number of that frame: AGC_EXTRA + batch_seq * wave_batch
+    int32_t n_batches;               // batches of this run (0 = none)
+    int32_t ring_pos0;               // ring entry of the run's first batch; < 0: resident run, the ring is left alone
+};
+struct ActArgs {
+    const ActCfg* cfg;  // [devices with the detector on]
+    const ActRun* run;
+    const float2* tw1;
+    const float2* tw2;
+    int wave_batch;
+};
+cudaError_t abg_launch_activity(int fft_size, const ActArgs& a, int n_devices, int max_batches, cudaStream_t s);
+
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B
     int lanes_per_warp;       // channels handled by one warp of K2: 1, 2, 4, 8, 16 or 32

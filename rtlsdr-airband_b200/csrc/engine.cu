@@ -169,7 +169,7 @@ struct DevBuf {
 };
 
 // Result queue of one device's batch monitor (band spectrum, carrier meter, input level meter, sub-band output, tone
-// meter).  The monitor's kernel writes the result of every batch straight into a page-locked, mapped ring of `cap` =
+// meter, activity detector).  The monitor's kernel writes the result of every batch straight into a page-locked, mapped ring of `cap` =
 // max_batches_per_run + 2 entries; the host keeps the unfetched entries, oldest first.  Lossy by design: queueing a run
 // drops the oldest unfetched entries beyond the ring's size (gaps show in their batch_seq), so a monitor never holds a
 // result slot or causes ABG_EOVERFLOW.
@@ -286,6 +286,10 @@ struct Device {
     // CTCSS tone meter (abg_tone_meter_configure); nothing is allocated until it is first switched on
     bool tm_on = false;
     MonitorQueue tm_q;               // S float[C][K][2], E float[C], active int32[C] per entry (room for ABG_TONE_MAX), Entry.aux = K
+    // band activity detector (abg_activity_configure); nothing is allocated until it is first switched on
+    int act_stride = 0, act_hang = 0, act_min_span = 0, act_n_sel = 0;
+    float* act_thr = nullptr;        // device [N] thresholds; kept once allocated
+    MonitorQueue act_q;              // head int32[4] {n_total, stride, hang, min_span}, then abg_burst[ABG_ACTIVITY_MAX_RECORDS]
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -420,12 +424,14 @@ struct abg_engine {
     cudaEvent_t tl[TL_RUNS][5] = {};
     bool tev_valid = false;
     std::vector<int32_t> h_bins;
-    // batch monitors: the first four are launched in this order on stream A after K1, the tone meter on stream B after K2
+    // batch monitors: the first four and the activity detector are launched in this order on stream A after K1, the tone
+    // meter on stream B after K2
     MonitorLaunch<SpecCfg, SpecRun> spectrum{"spectrum", true};
     MonitorLaunch<CarCfg, CarRun> carrier{"carrier meter", false};
     MonitorLaunch<InmCfg, InmRun> input_meter{"input meter", true};
     MonitorLaunch<SbCfg, SbRun> subband{"sub-band", true};
     MonitorLaunch<TmCfg, TmRun> tone_meter{"tone meter", false};
+    MonitorLaunch<ActCfg, ActRun> activity{"activity detector", true};
     // tone meter tables: the engine-wide tone list and, once the meter is first switched on, its [B][tm_cols] table
     std::vector<float> tm_freqs{std::begin(kStandardTones), std::end(kStandardTones)};
     std::vector<uint32_t> tm_delta;
@@ -558,6 +564,8 @@ void engine_free(abg_engine* e) {
         d.car_q.release();
         d.inm_q.release();
         d.tm_q.release();
+        if (d.act_thr) cudaFree(d.act_thr);
+        d.act_q.release();
         for (auto& so : d.sb) {
             if (so.coef) cudaFree(so.coef);
             so.q.release();
@@ -568,6 +576,7 @@ void engine_free(abg_engine* e) {
     monitor_free(e->input_meter);
     monitor_free(e->subband);
     monitor_free(e->tone_meter);
+    monitor_free(e->activity);
     e->tm_table.free();
     e->tm_chan_dev.free();
     for (auto& g : e->groups) {
@@ -1096,9 +1105,11 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     CU(cudaEventRecord(tl[1], sa));
     CU(cudaEventRecord(e->ev_k1[cur], sa));
     // ---- batch monitors (stream A after K1 in this order: the spectrum, the carrier meter, the input meter, the sub-band
-    // outputs; K2 does not wait for them past ev_k1).  Injected batches have no frames and launch none. ----
+    // outputs, the activity detector; K2 does not wait for them past ev_k1).  Injected batches have no frames and launch
+    // none. ----
     const int t = (int)(ri % TL_RUNS);
     e->spectrum.ran[t] = e->carrier.ran[t] = e->input_meter.ran[t] = e->subband.ran[t] = e->tone_meter.ran[t] = false;
+    e->activity.ran[t] = false;
     if (!skip_k1) {
         int max_items = 0;
         for (size_t m = 0; m < e->spectrum.devs.size(); m++) {
@@ -1176,6 +1187,24 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             SbArgs A{};
             A.cfg = e->subband.cfg.p; A.run = e->subband.run.p;
             return abg_launch_subband(A, n_devices, items, e->sb_max_hist, s);
+        });
+        if (rc != ABG_OK) return rc;
+        max_items = 0;
+        for (size_t m = 0; m < e->activity.devs.size(); m++) {
+            Device& d = e->dev[e->activity.devs[m]];
+            const int n = nb[e->activity.devs[m]];
+            ActRun& r = e->activity.h_run[m];
+            r.raw = resident ? d.res : d.raw[d.cur];
+            r.first_byte = run_first_byte(d, resident);
+            r.first_frame = (unsigned long long)ABG_AGC_EXTRA + d.batch_seq * (unsigned long long)B;
+            r.n_batches = n;
+            r.ring_pos0 = queue_outputs && n > 0 ? d.act_q.queue(n, d.batch_seq, ri, 0) : -1;
+            max_items = std::max(max_items, n);
+        }
+        rc = monitor_launch(e, e->activity, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+            ActArgs A{};
+            A.cfg = e->activity.cfg.p; A.run = e->activity.run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
+            return abg_launch_activity(N, A, n_devices, items, s);
         });
         if (rc != ABG_OK) return rc;
     }
@@ -1886,6 +1915,89 @@ int abg_fetch_tone_meter(abg_engine* e, int dev, float* tones, float* energy, in
 }
 
 int abg_debug_tone_meter_time(abg_engine* e, float* ms) { return monitor_time(e, e->tone_meter, ms, __func__); }
+
+// ---- band activity detector (definition in airband_b200.h) ----------------------------------------------------------
+int abg_activity_configure(abg_engine* e, int dev, int stride, int hang, int min_span, const float* thr) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_activity_configure: device %d out of range", dev);
+    if (stride < 0 || hang < 0 || min_span < 0)
+        return fail(ABG_EINVAL, "abg_activity_configure: negative argument (stride %d, hang %d, min_span %d)", stride, hang, min_span);
+    const int N = e->N, B = e->B, nbmax = e->nbmax;
+    if (stride > 0) {
+        if (stride > B) return fail(ABG_EINVAL, "abg_activity_configure: stride %d exceeds the batch of %d frames", stride, B);
+        const int n_sel = (B + stride - 1) / stride;
+        if (hang >= n_sel) return fail(ABG_EINVAL, "abg_activity_configure: hang %d is not below the %d selected frames of a batch", hang, n_sel);
+        if (min_span < 1) return fail(ABG_EINVAL, "abg_activity_configure: min_span %d is below 1", min_span);
+        if (!thr) return fail(ABG_EINVAL, "abg_activity_configure: null thresholds");
+        for (int k = 0; k < N; k++)
+            if (!std::isfinite(thr[k]) || !(thr[k] > 0.0f))
+                return fail(ABG_EINVAL, "abg_activity_configure: threshold of bin %d (%g) is not finite and positive", k, (double)thr[k]);
+    }
+    Device& d = e->dev[dev];
+    if (stride == 0 && d.act_stride == 0) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream));  // an enqueued detector kernel may still read the thresholds and the tables
+    if (stride > 0) {
+        if (monitor_on(e, e->activity) != ABG_OK) return ABG_ECUDA;
+        if (!d.act_q.alloc(nbmax + 2, ABG_ACT_HEAD_BYTES + sizeof(abg_burst) * (size_t)ABG_ACTIVITY_MAX_RECORDS))
+            return fail(ABG_ENOMEM, "Out of page-locked host memory for the activity ring");
+        if (!d.act_thr && cudaMalloc((void**)&d.act_thr, sizeof(float) * N) != cudaSuccess) {
+            d.act_thr = nullptr;
+            return fail(ABG_ENOMEM, "Out of device memory for the activity thresholds of device %d", dev);
+        }
+        CU(cudaMemcpy(d.act_thr, thr, sizeof(float) * N, cudaMemcpyHostToDevice));
+        d.act_n_sel = (B + stride - 1) / stride;
+    }
+    d.act_stride = stride;
+    d.act_hang = stride > 0 ? hang : 0;
+    d.act_min_span = stride > 0 ? min_span : 0;
+    // rebuild the launch's device list and its static table
+    std::vector<int> devs;
+    std::vector<ActCfg> cfgs;
+    for (int i = 0; i < (int)e->dev.size(); i++) {
+        const Device& x = e->dev[i];
+        if (x.act_stride <= 0) continue;
+        ActCfg c{};
+        c.wsc = e->groups[x.group].wsc.p;
+        c.thr = x.act_thr;
+        CU(cudaHostGetDevicePointer((void**)&c.ring, x.act_q.ring, 0));
+        c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = x.act_stride; c.n_sel = x.act_n_sel;
+        c.hang = x.act_hang; c.min_span = x.act_min_span;
+        c.ring_cap = x.act_q.cap; c.entry_bytes = (int32_t)x.act_q.entry_bytes;
+        devs.push_back(i);
+        cfgs.push_back(c);
+    }
+    return monitor_publish(e, e->activity, devs, cfgs);
+}
+
+static_assert(sizeof(abg_burst) == 40, "abg_burst has a fixed 40-byte layout");
+
+int abg_fetch_activity(abg_engine* e, int dev, abg_burst* out, int cap, int32_t* n_stored, int32_t* n_total, uint64_t* batch_seq,
+                       int32_t* settings3) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_activity: device %d out of range", dev);
+    if (cap < 0) return fail(ABG_EINVAL, "abg_fetch_activity: cap %d is negative", cap);
+    const unsigned char* src = nullptr;
+    MonitorQueue::Entry r{};
+    const int rc = monitor_pop(e, e->dev[dev].act_q, e->activity, &src, &r);
+    if (rc <= 0) return rc;
+    int32_t head[4];
+    memcpy(head, src, sizeof(head));
+    const int stored = std::min(head[0], (int32_t)ABG_ACTIVITY_MAX_RECORDS);
+    if (out && cap > 0) {
+        std::vector<abg_burst> v(stored);
+        memcpy(v.data(), src + ABG_ACT_HEAD_BYTES, sizeof(abg_burst) * (size_t)stored);
+        std::sort(v.begin(), v.end(), [](const abg_burst& a, const abg_burst& b) {
+            return a.bin != b.bin ? a.bin < b.bin : a.first_frame < b.first_frame;
+        });
+        memcpy(out, v.data(), sizeof(abg_burst) * (size_t)std::min(stored, cap));
+    }
+    if (n_stored) *n_stored = stored;
+    if (n_total) *n_total = head[0];
+    if (batch_seq) *batch_seq = r.seq;
+    if (settings3) memcpy(settings3, head + 1, sizeof(int32_t) * 3);
+    return 1;
+}
+
+int abg_debug_activity_time(abg_engine* e, float* ms) { return monitor_time(e, e->activity, ms, __func__); }
 
 // ---- scan mode -------------------------------------------------------------------------------------------------------
 static ScanView scan_view(abg_engine* e) {

@@ -11,7 +11,7 @@ from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .config import CConfig, CSquelchStats, Config
+from .config import AGC_EXTRA, CConfig, CSquelchStats, Config
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_DIR = os.path.abspath(os.path.join(_HERE, "..", ".."))
@@ -28,11 +28,14 @@ SYMBOLS = [
     "abg_input_meter_configure", "abg_fetch_input_levels", "abg_debug_input_meter_time",
     "abg_subband_configure", "abg_fetch_subband", "abg_debug_subband_time",
     "abg_tone_meter_configure", "abg_tone_meter_set_tones", "abg_fetch_tone_meter", "abg_debug_tone_meter_time",
+    "abg_activity_configure", "abg_fetch_activity", "abg_debug_activity_time",
 ]
 
 SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
 SUBBAND_MAX_COEFFS = 4096  # ABG_SUBBAND_MAX_COEFFS
 TONE_MAX = 64              # ABG_TONE_MAX: tones in the tone meter's list
+ACTIVITY_MAX_RECORDS = 4096  # ABG_ACTIVITY_MAX_RECORDS: pieces one activity reading stores
+BURST_OPEN_START, BURST_OPEN_END = 1, 2  # ABG_BURST_OPEN_START / ABG_BURST_OPEN_END
 # the tone meter's default list: the reference's standard CTCSS tones (CTCSS::standard_tones, src/ctcss.cpp:87-89)
 STANDARD_TONES = (67.0, 69.3, 71.9, 74.4, 77.0, 79.7, 82.5, 85.4, 88.5, 91.5, 94.8, 97.4, 100.0, 103.5, 107.2, 110.9, 114.8,
                   118.8, 123.0, 127.3, 131.8, 136.5, 141.3, 146.2, 150.0, 151.4, 156.7, 159.8, 162.2, 165.5, 167.9, 171.3,
@@ -65,6 +68,26 @@ class CInputLevels(C.Structure):
         ("peak", C.c_float * 2),
         ("hist", (C.c_uint32 * 256) * 2),
     ]
+
+
+class CBurst(C.Structure):
+    """abg_burst: one piece (or, after merge_bursts, one burst) of the band activity detector (definition in airband_b200.h)."""
+    _fields_ = [
+        ("bin", C.c_int32),
+        ("flags", C.c_int32),
+        ("first_frame", C.c_uint64),
+        ("last_frame", C.c_uint64),
+        ("n_active", C.c_int32),
+        ("peak", C.c_float),
+        ("sum", C.c_float),
+        ("reserved", C.c_int32),
+    ]
+
+
+# numpy mirror of abg_burst: fetch_activity returns arrays of it, merge_bursts takes and returns them
+BURST_DTYPE = np.dtype({"names": [f for f, _ in CBurst._fields_],
+                        "formats": ["<i4", "<i4", "<u8", "<u8", "<i4", "<f4", "<f4", "<i4"],
+                        "offsets": [getattr(CBurst, f).offset for f, _ in CBurst._fields_], "itemsize": C.sizeof(CBurst)})
 
 
 class AbgError(RuntimeError):
@@ -143,6 +166,10 @@ def load():
     L.abg_fetch_tone_meter.restype = i
     L.abg_fetch_tone_meter.argtypes = [vp, i, vp, vp, vp, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
     L.abg_debug_tone_meter_time.restype, L.abg_debug_tone_meter_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_activity_configure.restype, L.abg_activity_configure.argtypes = i, [vp, i, i, i, i, vp]
+    L.abg_fetch_activity.restype = i
+    L.abg_fetch_activity.argtypes = [vp, i, vp, i, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_uint64), vp]
+    L.abg_debug_activity_time.restype, L.abg_debug_activity_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -445,6 +472,31 @@ class Engine:
         """ms of the tone meter kernel in the most recent run (CUDA events on the K2 stream); 0 if it metered nothing."""
         return self._kernel_time(self.L.abg_debug_tone_meter_time)
 
+    # ---- band activity detector -----------------------------------------------------------------------------------
+    def activity_configure(self, dev: int, stride: int, hang: int = 0, min_span: int = 1, thr=None) -> None:
+        """Every burst above thr[fft_size] (on the band spectrum's scale) in a device's band, per batch, at every
+        `stride`-th frame; `hang` and `min_span` in selected frames (definition in airband_b200.h).  stride = 0 switches it
+        off.  Applies to batches enqueued by later runs.  `activity_threshold` builds thr from fetched spectra."""
+        t = None if thr is None else np.ascontiguousarray(thr, dtype=np.float32)
+        self._chk(self.L.abg_activity_configure(self.h, dev, int(stride), int(hang), int(min_span), _ptr(t)))
+
+    def fetch_activity(self, dev: int) -> Optional[dict]:
+        """Oldest unfetched reading of a device, or None: a dict of pieces (BURST_DTYPE array sorted by (bin, first_frame)),
+        n_total (pieces found; more than len(pieces) means truncated), batch_seq, settings = (stride, hang, min_span) and
+        wave_batch (frames per batch, which merge_bursts needs).
+        Lossy: at most max_batches_per_run + 2 are kept per device."""
+        buf = np.empty(ACTIVITY_MAX_RECORDS, BURST_DTYPE)
+        ns, nt, seq = C.c_int32(0), C.c_int32(0), C.c_uint64(0)
+        st = np.zeros(3, np.int32)
+        if not self._chk(self.L.abg_fetch_activity(self.h, dev, _ptr(buf), buf.size, C.byref(ns), C.byref(nt), C.byref(seq), _ptr(st))):
+            return None
+        return dict(pieces=buf[:ns.value].copy(), n_total=int(nt.value), batch_seq=int(seq.value),
+                    settings=tuple(int(x) for x in st), wave_batch=self.B)
+
+    def activity_time(self) -> float:
+        """ms of the activity detector kernel in the most recent run (CUDA events on the K1 stream); 0 if it ran none."""
+        return self._kernel_time(self.L.abg_debug_activity_time)
+
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
         """mixers[m] = [(dev, chan, ampfactor, balance), ...]"""
@@ -678,3 +730,134 @@ def demodulate_all(cfg: Config, raws: List[np.ndarray], *, max_batches_per_run: 
         else:
             res.append((np.zeros((Cn, 0), np.float32), np.zeros((Cn, 0), np.complex64), np.zeros((0, Cn), np.uint8)))
     return res, e
+
+
+def activity_threshold(power, margin_db: float, half_width: int) -> np.ndarray:
+    """Per-bin thresholds for Engine.activity_configure from band spectra (Engine.fetch_spectrum powers, one [fft_size] or
+    several [n, fft_size], averaged): the running median of the power over +-half_width bins, times 10^(margin_db / 10),
+    float32.  The median runs in frequency order and its window is cut at the band edges rather than wrapped, so it follows
+    the passband roll-off of the SDR's filter there; the carriers it is meant to catch sit margin_db above their
+    neighbourhood's median, as long as a carrier is narrower than half the window.  Bins whose median is zero get the
+    smallest positive float32 times the margin, so every threshold is > 0."""
+    p = np.asarray(power, np.float64)
+    if p.ndim == 2:
+        p = p.mean(axis=0)
+    if p.ndim != 1 or half_width < 0:
+        raise ValueError("activity_threshold: power must be [fft_size] or [n, fft_size], half_width >= 0")
+    n = p.size
+    f = np.fft.fftshift(p)  # frequency order: the band edges at both ends
+    w = 2 * half_width + 1
+    padded = np.concatenate([np.full(half_width, np.nan), f, np.full(half_width, np.nan)])
+    med = np.nanmedian(np.lib.stride_tricks.sliding_window_view(padded, w), axis=1)
+    med = np.maximum(np.fft.ifftshift(med), float(np.finfo(np.float32).tiny))
+    thr = (med * 10.0 ** (margin_db / 10.0)).astype(np.float32)
+    assert thr.size == n
+    return np.maximum(thr, np.finfo(np.float32).tiny)
+
+
+def merge_bursts(readings) -> np.ndarray:
+    """Stitch the pieces of consecutive activity readings of one device (Engine.fetch_activity dicts, oldest first) into
+    bursts (definition in airband_b200.h): a piece with OPEN_END joins the same bin's OPEN_START piece of the next reading
+    when their gap is <= hang + 1 selected frames, then bursts shorter than min_span are dropped.  Pieces still open at the
+    last reading end there.  Returns a BURST_DTYPE array sorted by (bin, first_frame), flags 0; a joined burst's sum is the
+    float32 sum of its pieces' sums.  Raises ValueError on a gap in batch_seq, a change of settings or a truncated
+    reading."""
+    readings = list(readings)
+    out = []
+    if not readings:
+        return np.zeros(0, BURST_DTYPE)
+    s, h, m = readings[0]["settings"]
+    B = readings[0]["wave_batch"]
+    n_sel = -(-B // s)
+
+    def q_of(frame, seq):  # absolute selected index q = seq * n + i of frame f = AGC_EXTRA + seq * B + i * s
+        return seq * n_sel + (int(frame) - AGC_EXTRA - seq * B) // s
+
+    open_ = {}  # bin -> [record, q_first, q_last] of the burst that may still grow
+    for idx, r in enumerate(readings):
+        if tuple(r["settings"]) != (s, h, m):
+            raise ValueError(f"merge_bursts: reading {idx} has settings {tuple(r['settings'])}, the first {(s, h, m)}")
+        if idx and r["batch_seq"] != readings[idx - 1]["batch_seq"] + 1:
+            raise ValueError(f"merge_bursts: gap in batch_seq: {readings[idx - 1]['batch_seq']} then {r['batch_seq']}")
+        if r["n_total"] > len(r["pieces"]):
+            raise ValueError(f"merge_bursts: reading {idx} (batch_seq {r['batch_seq']}) is truncated: {len(r['pieces'])} of {r['n_total']} pieces")
+        seq = r["batch_seq"]
+        nxt = {}
+        for p in np.sort(r["pieces"], order=["bin", "first_frame"]):
+            k = int(p["bin"])
+            qf, ql = q_of(p["first_frame"], seq), q_of(p["last_frame"], seq)
+            cur = None
+            if p["flags"] & BURST_OPEN_START and k in open_ and qf - open_[k][2] <= h + 1:
+                cur = open_.pop(k)
+                rec = cur[0]
+                rec["last_frame"] = p["last_frame"]
+                rec["n_active"] += p["n_active"]
+                rec["peak"] = max(rec["peak"], p["peak"])
+                rec["sum"] = np.float32(np.float32(rec["sum"]) + np.float32(p["sum"]))
+                cur[2] = ql
+            else:
+                rec = p.copy()
+                rec["flags"] = 0
+                cur = [rec, qf, ql]
+            if p["flags"] & BURST_OPEN_END:
+                nxt[k] = cur
+            elif cur[2] - cur[1] + 1 >= m:
+                out.append(cur[0])
+        for cur in open_.values():  # not continued in this reading
+            if cur[2] - cur[1] + 1 >= m:
+                out.append(cur[0])
+        open_ = nxt
+    for cur in open_.values():
+        if cur[2] - cur[1] + 1 >= m:
+            out.append(cur[0])
+    res = np.array(out, BURST_DTYPE) if out else np.zeros(0, BURST_DTYPE)
+    return np.sort(res, order=["bin", "first_frame"])
+
+
+def group_transmissions(bursts, cfg: Config, dev: int, max_bin_gap: int = 1, centerfreq: Optional[float] = None) -> List[dict]:
+    """Group the bursts of one device (merge_bursts output) into transmissions: bursts whose bins are at most max_bin_gap
+    apart in frequency and whose frame spans overlap join, transitively, so a carrier's main lobe and its sidebands become
+    one transmission.  Bins are taken in frequency order, bin k at offset k (k < fft_size / 2) or k - fft_size bins from
+    the centre, the inverse of config.calc_bin's wrap; one bin is sample_rate // fft_size Hz as in calc_bin.  Per
+    transmission, oldest first: freq_hz = centerfreq + the bursts' power-weighted (by sum) mean offset in bins times the bin
+    width; bins = (lowest, highest) signed offset; first_frame, last_frame; start_s / end_s = those frames' first samples
+    (frame * hop / sample_rate, the device's stream time); peak; energy = the sum of the bursts' sums; n_bursts; and
+    monitored = a configured channel's bin lies in [lowest, highest].  centerfreq defaults to the Device's."""
+    b = np.asarray(bursts, BURST_DTYPE)
+    d = cfg.devices[dev]
+    centerfreq = d.centerfreq if centerfreq is None else centerfreq
+    N = cfg.fft_size
+    bin_hz = d.sample_rate // N
+    hop = cfg.hop(dev)
+    sb = np.where(b["bin"] < N // 2, b["bin"], b["bin"] - N).astype(np.int64)
+    parent = list(range(b.size))
+
+    def find(x):
+        while parent[x] != x:
+            parent[x] = parent[parent[x]]
+            x = parent[x]
+        return x
+
+    order = np.argsort(sb, kind="stable")
+    for ii, x in enumerate(order):  # neighbours in frequency: only bursts up to max_bin_gap bins higher
+        for y in order[ii + 1:]:
+            if sb[y] - sb[x] > max_bin_gap:
+                break
+            if b["first_frame"][x] <= b["last_frame"][y] and b["first_frame"][y] <= b["last_frame"][x]:
+                parent[find(x)] = find(y)
+    groups = {}
+    for x in range(b.size):
+        groups.setdefault(find(x), []).append(x)
+    chan_bins = [c.bin if c.bin < N // 2 else c.bin - N for c in d.channels]
+    out = []
+    for members in groups.values():
+        m = np.asarray(members)
+        w = b["sum"][m].astype(np.float64)
+        lo, hi = int(sb[m].min()), int(sb[m].max())
+        first, last = int(b["first_frame"][m].min()), int(b["last_frame"][m].max())
+        out.append(dict(freq_hz=float(centerfreq) + float(np.sum(w * sb[m]) / np.sum(w)) * bin_hz, bins=(lo, hi),
+                        first_frame=first, last_frame=last, start_s=first * hop / d.sample_rate, end_s=last * hop / d.sample_rate,
+                        peak=float(b["peak"][m].max()), energy=float(w.sum()), n_bursts=int(m.size),
+                        monitored=any(lo <= c <= hi for c in chan_bins)))
+    out.sort(key=lambda t: (t["first_frame"], t["freq_hz"]))
+    return out

@@ -2,7 +2,7 @@
 process, plus the monitor kernel's own CUDA-event time and K1 / K2.  The card name and power limit are read in the same
 call.
 
-    python tools/monitor_overhead.py --monitor {spectrum,carrier,input_meter,subband,tone_meter} [--workloads cfg2,cfg5] [--runs 40]
+    python tools/monitor_overhead.py --monitor {spectrum,carrier,input_meter,subband,tone_meter,activity} [--workloads cfg2,cfg5] [--runs 40]
                                      [--reps 3] [--out DIR]
 
 Legs:
@@ -13,6 +13,8 @@ Legs:
                output but write none to the host rings, so these times leave out the outputs' transfer to host memory.
   tone_meter   off, on for every device with the 51 standard tones.  As for the sub-band outputs, resident runs leave out
                the readings' transfer to host memory.
+  activity     off, the default stride, stride 1; hang 1, min_span 1 and a uniform threshold of ACT_THR (|X|^2) for every
+               bin.  Resident runs count pieces but store none, so these times leave out the records' transfer.
 
 Prints one JSON line per workload (and writes it to DIR/<monitor>_overhead.jsonl with --out).  It uses only public
 lib.Engine methods, so ABG_LIB_PATH can point it at another build of the library."""
@@ -32,10 +34,18 @@ from airband_b200 import lib  # noqa: E402
 
 NB = 4  # batches per run, as bench.py's resident leg
 DECIM, NTAPS = 32, 255  # sub-band outputs
+ACT_THR = 1.0e4  # activity detector threshold, on the band spectrum's scale
 
 
 def raw_bytes_per_run(cfg):
     return sum(NB * cfg.wave_batch * cfg.hop(d) * 2 * dv.bytes_per_sample for d, dv in enumerate(cfg.devices))
+
+
+def activity_configure(e, cfg, d, stride):
+    if stride == 0:
+        e.activity_configure(d, 0)
+    else:
+        e.activity_configure(d, stride, 1, 1, np.full(cfg.fft_size, ACT_THR, np.float32))
 
 
 def subband_configure(e, cfg, d, n_out):
@@ -79,6 +89,11 @@ MONITORS = {
                            "wout_bytes_read_per_run": NB * cfg.wave_batch * sum(len(d.channels) for d in cfg.devices) * 4,
                            "gemm_flop_per_run": 2 * NB * sum(len(d.channels) for d in cfg.devices) * cfg.wave_batch
                            * 2 * len(lib.STANDARD_TONES)}),
+    "activity": dict(
+        legs=lambda cfg: {"off": 0, "default_stride": lib.default_stride(cfg, 0), "stride_1": 1},
+        configure=activity_configure,
+        time="activity_time", time_key="activity_ms", setting_key="stride",
+        extra=lambda cfg: {"threshold": ACT_THR, "hang": 1, "min_span": 1}),
 }
 
 
