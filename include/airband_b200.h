@@ -467,6 +467,51 @@ ABG_API int abg_fetch_activity(abg_engine* e, int dev, abg_burst* out, int cap, 
  * (0 if that run detected nothing).  Waits for it. */
 ABG_API int abg_debug_activity_time(abg_engine* e, float* ms);
 
+/* I/Q history (not part of the reference surface: the activity detector reports a burst only after its batch has been
+ * demodulated, and a sub-band output starts at the first batch after it is configured, so without it nothing the detector
+ * finds could be captured; an SDR recorder would need a dongle of its own).  A device with the history on keeps its most
+ * recent raw samples in HBM, in ring format (never expanded to float), and any sub-band can be cut out of them later.
+ * Names as for the sub-band outputs: v[s] is the float32 level of absolute sample s (counted from the device's first pushed
+ * sample), and batch b covers the samples [s0, s0 + n), s0 = (AGC_EXTRA + b*WAVE_BATCH) * hop, n = WAVE_BATCH * hop.
+ *   What it holds: a device with the history on appends the samples [s0, s0 + n) of every batch that later abg_run calls
+ *     demodulate.  Those ranges tile the stream, so the history is always one contiguous range [first, end) of absolute
+ *     samples, at most the capacity long; the oldest samples are overwritten first.
+ *   Capture: abg_history_subband computes y[m] of the sub-band definition (same delta, same g[j] built on the host by the
+ *     same function, same summation order) from the stored samples.  For any m whose live sub-band output with the same
+ *     offset_hz, decimation and coefficients had all L taps after its start, the captured y[m] is bitwise equal to the live
+ *     one.  Every tap has to lie in the history: there is no zero fill.
+ * Computed on the GPU: one extra kernel per run appends the run's bytes, on the K1 stream after K1 and every other monitor of
+ * that stream (it re-reads the device's raw bytes, K2 does not wait for it); captures are enqueued on the same stream, so
+ * every append they read is ahead of them and every later one that would overwrite their samples queues behind them.  With
+ * every device off (the default) nothing is allocated, uploaded, launched or recorded.  Resident runs (abg_run_resident)
+ * append from the replay buffer, so that their cost can be measured, but leave the history empty: a capture never mixes
+ * replayed and streamed samples.  Batches fed through abg_debug_inject_wavein append nothing.  A scan-mode retune moves the
+ * centre frequency under the recorded samples: a capture across a retune mixes both tunings.
+ *
+ * abg_history_configure: n_batches = 0 switches the history off and frees it; n_batches > 0 gives a capacity of
+ * n_batches * WAVE_BATCH * hop samples (abg_hop) for batches enqueued by later abg_run calls.  A change of capacity empties
+ * the history; a call that changes nothing returns at once.  ABG_ERANGE for a bad device, ABG_EINVAL for a negative count,
+ * ABG_ENOMEM if the allocation fails (the history is then off).  Waits for the engine's K1 stream. */
+ABG_API int abg_history_configure(abg_engine* e, int dev, int n_batches);
+/* The range [*first, *end) of absolute samples the history holds once every run enqueued so far has finished (first == end:
+ * empty).  Does not wait. */
+ABG_API int abg_history_range(abg_engine* e, int dev, uint64_t* first, uint64_t* end);
+/* Copy the ring-format bytes of samples [first, first + n) into out[n * bytes per complex sample]: byte for byte what was
+ * pushed.  ABG_ERANGE if any of them lies outside the range, ABG_EINVAL for n < 0 or a null out.  Waits for the runs that
+ * appended them. */
+ABG_API int abg_history_raw(abg_engine* e, int dev, uint64_t first, int64_t n, void* out);
+/* Down-convert y[m], m in [first_m, first_m + n_out), from the history into iq[2 * n_out] (interleaved cf32, caller memory).
+ * ABG_EINVAL for arguments abg_subband_configure refuses with decim >= 1 (decim outside [1, WAVE_BATCH * hop], the offset,
+ * the coefficients), n_out < 1 or a null iq; ABG_ERANGE unless first_m * decim - (n_coeffs - 1) >= first and
+ * (first_m + n_out - 1) * decim < end.  Any n_out that fits is accepted (large requests are split internally).  Waits for
+ * the capture to finish. */
+ABG_API int abg_history_subband(abg_engine* e, int dev, double offset_hz, int decim, int n_coeffs, const float* coeffs,
+                                uint64_t first_m, int64_t n_out, float* iq);
+/* Measurement aid: ms2[0] = device time of the append kernel of the most recent run (0 if that run appended nothing; waits
+ * for it), ms2[1] = device time of the kernels of the most recent abg_history_subband (0 before the first), both from CUDA
+ * events on the K1 stream. */
+ABG_API int abg_debug_history_time(abg_engine* e, float* ms2);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

@@ -304,6 +304,35 @@ struct ActArgs {
 };
 cudaError_t abg_launch_activity(int fft_size, const ActArgs& a, int n_devices, int max_batches, cudaStream_t s);
 
+// I/Q history (history.cu): see abg_history_configure in include/airband_b200.h
+struct HiCfg {  // per device with the history on; written by abg_history_configure
+    unsigned char* ring;             // device [ring_bytes]: stream byte b at b mod ring_bytes
+    unsigned long long ring_bytes;   // a multiple of 16
+};
+struct HiRun {  // per device with the history on; uploaded with every run
+    const unsigned char* src;        // first byte this run appends (its address agrees with dst modulo 16)
+    unsigned long long dst;          // ring byte of src[0], < ring_bytes
+    unsigned long long n_bytes;      // bytes this run appends, at most ring_bytes (0 = none)
+};
+struct HiArgs {
+    const HiCfg* cfg;  // [devices with the history on]
+    const HiRun* run;
+};
+cudaError_t abg_launch_history_append(const HiArgs& a, int n_devices, int blocks_per_device, cudaStream_t s);
+int abg_history_blocks(unsigned long long max_bytes, int n_devices, int sm_count);  // append CTAs per device
+struct HiCapture {  // one capture launch: outputs [m0, m0 + n_out) of one device's history
+    const unsigned char* ring;
+    unsigned long long ring_bytes;
+    const float2* coef;      // [n_coeffs] g[j], as the sub-band outputs build them
+    float2* out;             // device [n_out]
+    long long m0;
+    int32_t n_out, decim, n_coeffs, sfmt;
+    uint32_t delta;
+    float scale;             // 1.0f / fullscale (S16, F32)
+    int32_t per_item, stage; // set by the launcher
+};
+cudaError_t abg_launch_history_capture(HiCapture c, cudaStream_t s);
+
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B
     int lanes_per_warp;       // channels handled by one warp of K2: 1, 2, 4, 8, 16 or 32

@@ -290,6 +290,12 @@ struct Device {
     int act_stride = 0, act_hang = 0, act_min_span = 0, act_n_sel = 0;
     float* act_thr = nullptr;        // device [N] thresholds; kept once allocated
     MonitorQueue act_q;              // head int32[4] {n_total, stride, hang, min_span}, then abg_burst[ABG_ACTIVITY_MAX_RECORDS]
+    // I/Q history (abg_history_configure); nothing is allocated until it is first switched on, and it is freed when off
+    int hi_batches = 0;                    // capacity in batches, 0 = off
+    unsigned char* hi_ring = nullptr;      // device [hi_ring_bytes]: stream byte b at b mod hi_ring_bytes
+    unsigned long long hi_ring_bytes = 0;  // hi_cap * bpc rounded up to a multiple of 16
+    unsigned long long hi_cap = 0;         // capacity in samples
+    unsigned long long hi_first = 0, hi_end = 0;  // samples [first, end) the ring holds once every enqueued run has finished
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -424,14 +430,19 @@ struct abg_engine {
     cudaEvent_t tl[TL_RUNS][5] = {};
     bool tev_valid = false;
     std::vector<int32_t> h_bins;
-    // batch monitors: the first four and the activity detector are launched in this order on stream A after K1, the tone
-    // meter on stream B after K2
+    // batch monitors: the first four, the activity detector and the I/Q history's append are launched in this order on
+    // stream A after K1, the tone meter on stream B after K2
     MonitorLaunch<SpecCfg, SpecRun> spectrum{"spectrum", true};
     MonitorLaunch<CarCfg, CarRun> carrier{"carrier meter", false};
     MonitorLaunch<InmCfg, InmRun> input_meter{"input meter", true};
     MonitorLaunch<SbCfg, SbRun> subband{"sub-band", true};
     MonitorLaunch<TmCfg, TmRun> tone_meter{"tone meter", false};
     MonitorLaunch<ActCfg, ActRun> activity{"activity detector", true};
+    MonitorLaunch<HiCfg, HiRun> history{"I/Q history", true};  // the append, last on stream A
+    // I/Q history captures: coefficient and output scratch (allocated by the first capture) and the last capture's kernel time
+    DevBuf<float2> hi_coef, hi_out;
+    cudaEvent_t hi_ev[2] = {nullptr, nullptr};
+    float hi_capture_ms = 0.0f;
     // tone meter tables: the engine-wide tone list and, once the meter is first switched on, its [B][tm_cols] table
     std::vector<float> tm_freqs{std::begin(kStandardTones), std::end(kStandardTones)};
     std::vector<uint32_t> tm_delta;
@@ -566,6 +577,7 @@ void engine_free(abg_engine* e) {
         d.tm_q.release();
         if (d.act_thr) cudaFree(d.act_thr);
         d.act_q.release();
+        if (d.hi_ring) cudaFree(d.hi_ring);
         for (auto& so : d.sb) {
             if (so.coef) cudaFree(so.coef);
             so.q.release();
@@ -577,6 +589,11 @@ void engine_free(abg_engine* e) {
     monitor_free(e->subband);
     monitor_free(e->tone_meter);
     monitor_free(e->activity);
+    monitor_free(e->history);
+    e->hi_coef.free();
+    e->hi_out.free();
+    for (auto& ev : e->hi_ev)
+        if (ev) cudaEventDestroy(ev);
     e->tm_table.free();
     e->tm_chan_dev.free();
     for (auto& g : e->groups) {
@@ -1109,7 +1126,7 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     // none. ----
     const int t = (int)(ri % TL_RUNS);
     e->spectrum.ran[t] = e->carrier.ran[t] = e->input_meter.ran[t] = e->subband.ran[t] = e->tone_meter.ran[t] = false;
-    e->activity.ran[t] = false;
+    e->activity.ran[t] = e->history.ran[t] = false;
     if (!skip_k1) {
         int max_items = 0;
         for (size_t m = 0; m < e->spectrum.devs.size(); m++) {
@@ -1205,6 +1222,38 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
             ActArgs A{};
             A.cfg = e->activity.cfg.p; A.run = e->activity.run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
             return abg_launch_activity(N, A, n_devices, items, s);
+        });
+        if (rc != ABG_OK) return rc;
+        // the I/Q history's append: the run's samples [s0, s0 + n) of every device with the history on, at most the last
+        // ring-full of them.  Resident runs append from the replay buffer at its own offsets and leave the history empty.
+        unsigned long long max_bytes = 0;
+        for (size_t m = 0; m < e->history.devs.size(); m++) {
+            Device& d = e->dev[e->history.devs[m]];
+            const int n = nb[e->history.devs[m]];
+            HiRun& r = e->history.h_run[m];
+            const unsigned long long first_byte = run_first_byte(d, resident);
+            const unsigned long long stream_byte = (resident ? 0ull : (unsigned long long)d.dropped) + first_byte;
+            const unsigned long long bytes = (unsigned long long)n * B * d.hop_bytes, R = d.hi_ring_bytes;
+            const unsigned long long skip = bytes > R ? bytes - R : 0;
+            r.src = (resident ? d.res : d.raw[d.cur]) + first_byte + skip;
+            r.dst = (stream_byte + skip) % R;
+            r.n_bytes = bytes - skip;
+            max_bytes = std::max(max_bytes, r.n_bytes);
+            if (n == 0) continue;
+            if (resident) {
+                d.hi_first = d.hi_end = 0;
+                continue;
+            }
+            const unsigned long long s0 = stream_byte / d.bpc;
+            if (d.hi_first == d.hi_end || s0 != d.hi_end) d.hi_first = s0;
+            d.hi_end = s0 + (unsigned long long)n * B * d.hop;
+            if (d.hi_end - d.hi_first > d.hi_cap) d.hi_first = d.hi_end - d.hi_cap;
+        }
+        max_items = max_bytes > 0 ? abg_history_blocks(max_bytes, (int)e->history.devs.size(), e->sm_count) : 0;
+        rc = monitor_launch(e, e->history, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+            HiArgs A{};
+            A.cfg = e->history.cfg.p; A.run = e->history.run.p;
+            return abg_launch_history_append(A, n_devices, items, s);
         });
         if (rc != ABG_OK) return rc;
     }
@@ -1379,8 +1428,8 @@ int abg_push(abg_engine* e, int dev, const void* iq, size_t nbytes) {
         }
         // the destination buffer was last read by a K1 launched before the previous compaction: with at least one run since
         // then that is run_index-2 or older, so the copy overlaps the K1 that is reading the current buffer right now
-        // (the band spectrum, the input meter and the sub-band outputs read the same bytes right after that K1: ev_raw
-        // follows the last of them)
+        // (the band spectrum, the input meter, the sub-band outputs, the activity detector and the I/Q history's append read
+        // the same bytes right after that K1: ev_raw follows the last of them)
         if (d.runs_since_compaction >= 1) {
             if (e->run_index >= 2) {
                 CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 2) & 1], 0));
@@ -1711,6 +1760,31 @@ int abg_fetch_input_levels(abg_engine* e, int dev, abg_input_levels* out) {
 int abg_debug_input_meter_time(abg_engine* e, float* ms) { return monitor_time(e, e->input_meter, ms, __func__); }
 
 // ---- sub-band I/Q outputs (definition in airband_b200.h) ---------------------------------------------------------------
+// The arguments of a down-converter that is on (decim >= 1), as abg_subband_configure and abg_history_subband accept them.
+static int subband_check(const char* fn, const Device& d, int batch_samples, double offset_hz, int decim, int n_coeffs, const float* coeffs) {
+    if (decim < 1 || decim > batch_samples) return fail(ABG_EINVAL, "%s: decimation %d outside [1, %d]", fn, decim, batch_samples);
+    if (!std::isfinite(offset_hz) || fabs(offset_hz) > d.sample_rate / 2.0)
+        return fail(ABG_EINVAL, "%s: offset %g Hz outside +-sample_rate/2", fn, offset_hz);
+    if (n_coeffs < 1 || n_coeffs > ABG_SUBBAND_MAX_COEFFS)
+        return fail(ABG_EINVAL, "%s: %d coefficients outside [1, %d]", fn, n_coeffs, ABG_SUBBAND_MAX_COEFFS);
+    if (!coeffs) return fail(ABG_EINVAL, "%s: null coefficients", fn);
+    for (int j = 0; j < n_coeffs; j++)
+        if (!std::isfinite(coeffs[j])) return fail(ABG_EINVAL, "%s: coefficient %d is not finite", fn, j);
+    return ABG_OK;
+}
+
+// delta = llround(offset / fs * 2^32) mod 2^32; g[j] = h[j] exp(+2 pi i delta j / 2^32) in double, then float32
+static uint32_t subband_coefficients(double offset_hz, int sample_rate, int n_coeffs, const float* coeffs, std::vector<float2>& g) {
+    const uint32_t delta = (uint32_t)(unsigned long long)llround(offset_hz / sample_rate * 4294967296.0);
+    g.resize(n_coeffs);
+    for (int j = 0; j < n_coeffs; j++) {
+        const double turns = (double)(int32_t)(delta * (uint32_t)j) * 0x1p-32;  // exact, in [-1/2, 1/2)
+        const double a = 2.0 * M_PI * turns;
+        g[j] = make_float2((float)(coeffs[j] * cos(a)), (float)(coeffs[j] * sin(a)));
+    }
+    return delta;
+}
+
 int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int decim, int n_coeffs, const float* coeffs) {
     if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_subband_configure: device %d out of range", dev);
     if (k < 0 || k >= ABG_SUBBAND_MAX) return fail(ABG_ERANGE, "abg_subband_configure: output %d out of range [0, %d)", k, ABG_SUBBAND_MAX);
@@ -1718,13 +1792,8 @@ int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int d
     const int n = e->B * d.hop;  // samples per batch
     if (decim < 0 || decim > n) return fail(ABG_EINVAL, "abg_subband_configure: decimation %d outside [0, %d]", decim, n);
     if (decim > 0) {
-        if (!std::isfinite(offset_hz) || fabs(offset_hz) > d.sample_rate / 2.0)
-            return fail(ABG_EINVAL, "abg_subband_configure: offset %g Hz outside +-sample_rate/2", offset_hz);
-        if (n_coeffs < 1 || n_coeffs > ABG_SUBBAND_MAX_COEFFS)
-            return fail(ABG_EINVAL, "abg_subband_configure: %d coefficients outside [1, %d]", n_coeffs, ABG_SUBBAND_MAX_COEFFS);
-        if (!coeffs) return fail(ABG_EINVAL, "abg_subband_configure: null coefficients");
-        for (int j = 0; j < n_coeffs; j++)
-            if (!std::isfinite(coeffs[j])) return fail(ABG_EINVAL, "abg_subband_configure: coefficient %d is not finite", j);
+        const int rc = subband_check("abg_subband_configure", d, n, offset_hz, decim, n_coeffs, coeffs);
+        if (rc != ABG_OK) return rc;
     }
     Device::Subband& so = d.sb[k];
     if (decim == 0 && !so.on) return ABG_OK;
@@ -1732,14 +1801,8 @@ int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int d
     CU(cudaStreamSynchronize(e->stream));  // an enqueued kernel may still read the tables, the coefficients or the ring
     if (decim > 0) {
         if (monitor_on(e, e->subband) != ABG_OK) return ABG_ECUDA;
-        // delta = llround(offset / fs * 2^32) mod 2^32; g[j] = h[j] exp(+2 pi i delta j / 2^32) in double, then float32
-        const uint32_t delta = (uint32_t)(unsigned long long)llround(offset_hz / d.sample_rate * 4294967296.0);
-        std::vector<float2> g(n_coeffs);
-        for (int j = 0; j < n_coeffs; j++) {
-            const double turns = (double)(int32_t)(delta * (uint32_t)j) * 0x1p-32;  // exact, in [-1/2, 1/2)
-            const double a = 2.0 * M_PI * turns;
-            g[j] = make_float2((float)(coeffs[j] * cos(a)), (float)(coeffs[j] * sin(a)));
-        }
+        std::vector<float2> g;
+        const uint32_t delta = subband_coefficients(offset_hz, d.sample_rate, n_coeffs, coeffs, g);
         if (so.coef_cap < n_coeffs) {
             if (so.coef) cudaFree(so.coef);
             so.coef = nullptr;
@@ -1998,6 +2061,140 @@ int abg_fetch_activity(abg_engine* e, int dev, abg_burst* out, int cap, int32_t*
 }
 
 int abg_debug_activity_time(abg_engine* e, float* ms) { return monitor_time(e, e->activity, ms, __func__); }
+
+// ---- I/Q history (definition in airband_b200.h) ---------------------------------------------------------------------
+constexpr long long kHistoryCaptureChunk = 1 << 20;  // outputs per capture launch: the output scratch is 8 MB
+
+int abg_history_configure(abg_engine* e, int dev, int n_batches) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_configure: device %d out of range", dev);
+    if (n_batches < 0) return fail(ABG_EINVAL, "abg_history_configure: n_batches %d is negative", n_batches);
+    Device& d = e->dev[dev];
+    if (n_batches == d.hi_batches) return ABG_OK;
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(e->stream));  // an enqueued append or capture may still use the ring and the tables
+    if (d.hi_ring) cudaFree(d.hi_ring);
+    d.hi_ring = nullptr;
+    d.hi_batches = 0;
+    d.hi_ring_bytes = d.hi_cap = d.hi_first = d.hi_end = 0;
+    int rc = ABG_OK;
+    if (n_batches > 0) {
+        if (monitor_on(e, e->history) != ABG_OK) return ABG_ECUDA;
+        const unsigned long long cap = (unsigned long long)n_batches * e->B * d.hop;
+        const unsigned long long R = (cap * d.bpc + 15) & ~15ull;
+        if (cudaMalloc((void**)&d.hi_ring, R) != cudaSuccess) {
+            cudaGetLastError();  // not sticky: keep it from failing the next launch check
+            d.hi_ring = nullptr;
+            rc = fail(ABG_ENOMEM, "Out of device memory for the I/Q history of device %d (%llu bytes)", dev, R);
+        } else {
+            d.hi_batches = n_batches;
+            d.hi_cap = cap;
+            d.hi_ring_bytes = R;
+        }
+    }
+    // rebuild the launch's device list and its static table
+    std::vector<int> devs;
+    std::vector<HiCfg> cfgs;
+    for (int i = 0; i < (int)e->dev.size(); i++) {
+        const Device& x = e->dev[i];
+        if (!x.hi_ring) continue;
+        HiCfg c{};
+        c.ring = x.hi_ring;
+        c.ring_bytes = x.hi_ring_bytes;
+        devs.push_back(i);
+        cfgs.push_back(c);
+    }
+    const int rp = monitor_publish(e, e->history, devs, cfgs);
+    return rc != ABG_OK ? rc : rp;
+}
+
+int abg_history_range(abg_engine* e, int dev, uint64_t* first, uint64_t* end) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_range: device %d out of range", dev);
+    if (!first || !end) return fail(ABG_EINVAL, "abg_history_range: null argument");
+    *first = e->dev[dev].hi_first;
+    *end = e->dev[dev].hi_end;
+    return ABG_OK;
+}
+
+// [first, first + n) inside the device's history (n >= 1)
+static bool history_holds(const Device& d, unsigned __int128 first, unsigned __int128 n) {
+    return d.hi_first < d.hi_end && first >= d.hi_first && first + n <= d.hi_end;
+}
+
+int abg_history_raw(abg_engine* e, int dev, uint64_t first, int64_t n, void* out) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_raw: device %d out of range", dev);
+    if (n < 0 || (n > 0 && !out)) return fail(ABG_EINVAL, "abg_history_raw: %lld samples into %p", (long long)n, out);
+    const Device& d = e->dev[dev];
+    if (n == 0) return ABG_OK;
+    if (!history_holds(d, first, (unsigned long long)n))
+        return fail(ABG_ERANGE, "abg_history_raw: samples [%llu, +%lld) outside the history [%llu, %llu)", (unsigned long long)first,
+                    (long long)n, (unsigned long long)d.hi_first, (unsigned long long)d.hi_end);
+    cudaSetDevice(e->cuda_dev);
+    // on the K1 stream, behind the appends that wrote them; n <= capacity, so at most one wrap
+    const unsigned long long R = d.hi_ring_bytes, b0 = (unsigned long long)first * d.bpc % R, len = (unsigned long long)n * d.bpc;
+    const unsigned long long len0 = std::min(len, R - b0);
+    CU(cudaMemcpyAsync(out, d.hi_ring + b0, len0, cudaMemcpyDeviceToHost, e->stream));
+    if (len0 < len) CU(cudaMemcpyAsync(static_cast<char*>(out) + len0, d.hi_ring, len - len0, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    return ABG_OK;
+}
+
+int abg_history_subband(abg_engine* e, int dev, double offset_hz, int decim, int n_coeffs, const float* coeffs, uint64_t first_m,
+                        int64_t n_out, float* iq) {
+    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_subband: device %d out of range", dev);
+    const Device& d = e->dev[dev];
+    int rc = subband_check("abg_history_subband", d, e->B * d.hop, offset_hz, decim, n_coeffs, coeffs);
+    if (rc != ABG_OK) return rc;
+    if (n_out < 1 || !iq) return fail(ABG_EINVAL, "abg_history_subband: %lld outputs into %p", (long long)n_out, (void*)iq);
+    // every tap in the history: first_m D - (L - 1) >= first and (first_m + n_out - 1) D < end
+    const unsigned __int128 D = (unsigned)decim, lo = (unsigned __int128)first_m * D, hi = ((unsigned __int128)first_m + n_out - 1) * D;
+    if (d.hi_first == d.hi_end || lo < (unsigned __int128)d.hi_first + (n_coeffs - 1) || hi >= d.hi_end)
+        return fail(ABG_ERANGE, "abg_history_subband: outputs [%llu, +%lld) at decimation %d with %d coefficients read samples outside the history [%llu, %llu)",
+                    (unsigned long long)first_m, (long long)n_out, decim, n_coeffs, (unsigned long long)d.hi_first, (unsigned long long)d.hi_end);
+    std::vector<float2> g;
+    const uint32_t delta = subband_coefficients(offset_hz, d.sample_rate, n_coeffs, coeffs, g);
+    cudaSetDevice(e->cuda_dev);
+    if (!e->hi_out.p) {
+        if (e->hi_coef.alloc(ABG_SUBBAND_MAX_COEFFS) || e->hi_out.alloc(kHistoryCaptureChunk)) {
+            cudaGetLastError();
+            e->hi_coef.free();
+            e->hi_out.free();
+            return fail(ABG_ENOMEM, "Out of device memory for the I/Q history capture");
+        }
+        for (auto& ev : e->hi_ev) CU(cudaEventCreate(&ev));
+    }
+    // on the K1 stream: behind every append it reads, and ahead of every later one that would overwrite its samples
+    CU(cudaMemcpyAsync(e->hi_coef.p, g.data(), sizeof(float2) * n_coeffs, cudaMemcpyHostToDevice, e->stream));
+    HiCapture c{};
+    c.ring = d.hi_ring; c.ring_bytes = d.hi_ring_bytes; c.coef = e->hi_coef.p; c.out = e->hi_out.p;
+    c.decim = decim; c.n_coeffs = n_coeffs; c.sfmt = d.sfmt; c.delta = delta; c.scale = 1.0f / d.fullscale;
+    float total_ms = 0.0f;
+    for (long long done = 0; done < n_out;) {
+        const long long cnt = std::min<long long>(kHistoryCaptureChunk, n_out - done);
+        c.m0 = (long long)(first_m + (uint64_t)done);
+        c.n_out = (int32_t)cnt;
+        CU(cudaEventRecord(e->hi_ev[0], e->stream));
+        const cudaError_t er = abg_launch_history_capture(c, e->stream);
+        if (er != cudaSuccess) return fail(ABG_ECUDA, "I/Q history capture launch failed: %s", cudaGetErrorString(er));
+        e->launches++;
+        CU(cudaEventRecord(e->hi_ev[1], e->stream));
+        CU(cudaMemcpyAsync(iq + 2 * done, e->hi_out.p, sizeof(float2) * cnt, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaStreamSynchronize(e->stream));
+        float ms = 0.0f;
+        CU(cudaEventElapsedTime(&ms, e->hi_ev[0], e->hi_ev[1]));
+        total_ms += ms;
+        done += cnt;
+    }
+    e->hi_capture_ms = total_ms;
+    return ABG_OK;
+}
+
+int abg_debug_history_time(abg_engine* e, float* ms2) {
+    if (!ms2) return fail(ABG_EINVAL, "abg_debug_history_time: null argument");
+    const int rc = monitor_time(e, e->history, ms2, __func__);
+    if (rc != ABG_OK) return rc;
+    ms2[1] = e->hi_capture_ms;
+    return ABG_OK;
+}
 
 // ---- scan mode -------------------------------------------------------------------------------------------------------
 static ScanView scan_view(abg_engine* e) {

@@ -24,6 +24,7 @@
 
 #include "../../include/airband_b200.h"
 #include "abg_internal.h"
+#include "subband_dsp.cuh"
 
 namespace {
 
@@ -41,56 +42,6 @@ __device__ __forceinline__ long long ceil_div(long long a, long long b) {  // a 
     return (a + b - 1) / b;
 }
 
-// One complex sample at p (2, 4 or 8 bytes, aligned to its size): the input meter's float32 levels
-template <int SFMT>
-__device__ __forceinline__ float2 level(const unsigned char* p, float scale, const float* lut8) {
-    if constexpr (SFMT == ABG_SFMT_U8) {
-        const uchar2 c = *reinterpret_cast<const uchar2*>(p);
-        return make_float2(lut8[c.x], lut8[c.y]);
-    } else if constexpr (SFMT == ABG_SFMT_S8) {
-        const char2 c = *reinterpret_cast<const char2*>(p);
-        return make_float2(__fmul_rn((float)c.x, 0.0078125f), __fmul_rn((float)c.y, 0.0078125f));  // c / 128.0f, exact
-    } else if constexpr (SFMT == ABG_SFMT_S16) {
-        const short2 x = *reinterpret_cast<const short2*>(p);
-        return make_float2(__fmul_rn(scale, (float)x.x), __fmul_rn(scale, (float)x.y));
-    } else {
-        const float2 x = *reinterpret_cast<const float2*>(p);
-        return make_float2(__fmul_rn(scale, x.x), __fmul_rn(scale, x.y));
-    }
-}
-
-// 16 bytes that start with an I component -> 16 / bpc samples at dst (16-byte aligned)
-template <int SFMT>
-__device__ __forceinline__ void level_vec(uint4 q, float scale, const float* lut8, float2* dst) {
-    float4* d4 = reinterpret_cast<float4*>(dst);
-    if constexpr (SFMT == ABG_SFMT_U8 || SFMT == ABG_SFMT_S8) {
-        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {  // two samples per word: I0 Q0 I1 Q1
-            float c[4];
-#pragma unroll
-            for (int b = 0; b < 4; ++b) {
-                const uint32_t code = (w[i] >> (8 * b)) & 0xffu;
-                c[b] = SFMT == ABG_SFMT_U8 ? lut8[code] : __fmul_rn((float)(signed char)code, 0.0078125f);
-            }
-            d4[i] = make_float4(c[0], c[1], c[2], c[3]);
-        }
-    } else if constexpr (SFMT == ABG_SFMT_S16) {
-        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-        float c[8];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            c[2 * i] = __fmul_rn(scale, (float)(short)(w[i] & 0xffffu));
-            c[2 * i + 1] = __fmul_rn(scale, (float)(short)(w[i] >> 16));
-        }
-        d4[0] = make_float4(c[0], c[1], c[2], c[3]);
-        d4[1] = make_float4(c[4], c[5], c[6], c[7]);
-    } else {
-        d4[0] = make_float4(__fmul_rn(scale, __uint_as_float(q.x)), __fmul_rn(scale, __uint_as_float(q.y)),
-                            __fmul_rn(scale, __uint_as_float(q.z)), __fmul_rn(scale, __uint_as_float(q.w)));
-    }
-}
-
 template <int SFMT>
 __device__ void subband_item(const SbCfg& cf, const SbRun& rn, int k, int c, unsigned char* smem) {
     constexpr int BPC = SFMT == ABG_SFMT_F32 ? 8 : SFMT == ABG_SFMT_S16 ? 4 : 2;  // bytes per complex sample
@@ -101,7 +52,7 @@ __device__ void subband_item(const SbCfg& cf, const SbRun& rn, int k, int c, uns
     float* lut8 = reinterpret_cast<float*>(tile + TILE);
     if constexpr (SFMT == ABG_SFMT_U8) {
         static_assert(BLOCK == 256, "one thread per U8 code");
-        lut8[tid] = __fdiv_rn(__fsub_rn((float)tid, 127.5f), 127.5f);
+        sb_lut8_fill(lut8, tid);
         __syncthreads();
     }
     const float scale = cf.scale;
@@ -119,10 +70,10 @@ __device__ void subband_item(const SbCfg& cf, const SbRun& rn, int k, int c, uns
     const int n_head = (int)(v_lo - a_lo), n_tail = (int)(a_hi - v_hi), n_vec = (int)((v_hi - v_lo) / SPV);
     if (tid < n_head) {
         const long long a = a_lo + tid;
-        sv[a - a_org] = a < rn.base ? make_float2(0.0f, 0.0f) : level<SFMT>(raw + (a - rn.base) * BPC, scale, lut8);
+        sv[a - a_org] = a < rn.base ? make_float2(0.0f, 0.0f) : sb_level<SFMT>(raw + (a - rn.base) * BPC, scale, lut8);
     } else if (tid >= 32 && tid - 32 < n_tail) {
         const long long a = v_hi + (tid - 32);
-        sv[a - a_org] = a < rn.base ? make_float2(0.0f, 0.0f) : level<SFMT>(raw + (a - rn.base) * BPC, scale, lut8);
+        sv[a - a_org] = a < rn.base ? make_float2(0.0f, 0.0f) : sb_level<SFMT>(raw + (a - rn.base) * BPC, scale, lut8);
     }
 #pragma unroll 4
     for (int i = tid; i < n_vec; i += BLOCK) {
@@ -132,7 +83,7 @@ __device__ void subband_item(const SbCfg& cf, const SbRun& rn, int k, int c, uns
 #pragma unroll
             for (int s = 0; s < SPV; ++s) dst[s] = make_float2(0.0f, 0.0f);
         } else {
-            level_vec<SFMT>(__ldg(reinterpret_cast<const uint4*>(raw + (a - rn.base) * BPC)), scale, lut8, dst);
+            sb_level_vec<SFMT>(__ldg(reinterpret_cast<const uint4*>(raw + (a - rn.base) * BPC)), scale, lut8, dst);
         }
     }
     __syncthreads();
@@ -160,31 +111,15 @@ __device__ void subband_item(const SbCfg& cf, const SbRun& rn, int k, int c, uns
                     const int jmax = (int)min((long long)L, x - start + 1);
                     float ar = 0.0f, ai = 0.0f;
 #pragma unroll 4
-                    for (int j = lane; j < jmax; j += 32) {
-                        const float2 h = __ldg(g + j), v = vx[-j];
-                        ar = __fmaf_rn(h.x, v.x, ar);
-                        ar = __fmaf_rn(-h.y, v.y, ar);
-                        ai = __fmaf_rn(h.x, v.y, ai);
-                        ai = __fmaf_rn(h.y, v.x, ai);
-                    }
-#pragma unroll
-                    for (int s = 16; s >= 1; s >>= 1) {
-                        ar = __fadd_rn(ar, __shfl_xor_sync(0xffffffffu, ar, s));
-                        ai = __fadd_rn(ai, __shfl_xor_sync(0xffffffffu, ai, s));
-                    }
+                    for (int j = lane; j < jmax; j += 32) sb_tap(__ldg(g + j), vx[-j], ar, ai);
+                    sb_xor_tree(ar, ai);
                     if (lane == q) {
                         yr = ar;
                         yi = ai;
                     }
                 }
                 if (lane < nq) {
-                    // exp(-2 pi i p / 2^32) with p = delta * x mod 2^32, as a signed turn fraction in [-1/2, 1/2)
-                    const long long x = (mt + i0 + lane) * D;
-                    const int32_t p = (int32_t)(so.delta * (uint32_t)(unsigned long long)x);
-                    double sn, cs;
-                    sincospi((double)p * 0x1p-31, &sn, &cs);
-                    const float cf32 = (float)cs, sf32 = (float)sn;
-                    tile[i0 + lane] = make_float2(__fmaf_rn(yr, cf32, __fmul_rn(yi, sf32)), __fmaf_rn(yi, cf32, -__fmul_rn(yr, sf32)));
+                    tile[i0 + lane] = sb_rotate(yr, yi, so.delta, (mt + i0 + lane) * D);
                 }
             }
             __syncthreads();

@@ -29,6 +29,7 @@ SYMBOLS = [
     "abg_subband_configure", "abg_fetch_subband", "abg_debug_subband_time",
     "abg_tone_meter_configure", "abg_tone_meter_set_tones", "abg_fetch_tone_meter", "abg_debug_tone_meter_time",
     "abg_activity_configure", "abg_fetch_activity", "abg_debug_activity_time",
+    "abg_history_configure", "abg_history_range", "abg_history_raw", "abg_history_subband", "abg_debug_history_time",
 ]
 
 SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
@@ -170,6 +171,13 @@ def load():
     L.abg_fetch_activity.restype = i
     L.abg_fetch_activity.argtypes = [vp, i, vp, i, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_uint64), vp]
     L.abg_debug_activity_time.restype, L.abg_debug_activity_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_history_configure.restype, L.abg_history_configure.argtypes = i, [vp, i, i]
+    L.abg_history_range.restype = i
+    L.abg_history_range.argtypes = [vp, i, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    L.abg_history_raw.restype, L.abg_history_raw.argtypes = i, [vp, i, C.c_uint64, C.c_int64, vp]
+    L.abg_history_subband.restype = i
+    L.abg_history_subband.argtypes = [vp, i, C.c_double, i, i, vp, C.c_uint64, C.c_int64, vp]
+    L.abg_debug_history_time.restype, L.abg_debug_history_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -496,6 +504,42 @@ class Engine:
     def activity_time(self) -> float:
         """ms of the activity detector kernel in the most recent run (CUDA events on the K1 stream); 0 if it ran none."""
         return self._kernel_time(self.L.abg_debug_activity_time)
+
+    # ---- I/Q history ----------------------------------------------------------------------------------------------
+    def history_configure(self, dev: int, n_batches: int) -> None:
+        """Keep a device's most recent n_batches * wave_batch * hop raw samples in HBM (definition in airband_b200.h), from
+        the batches of later runs on; 0 switches it off and frees it.  A change of capacity empties it."""
+        self._chk(self.L.abg_history_configure(self.h, dev, int(n_batches)))
+
+    def history_range(self, dev: int) -> Tuple[int, int]:
+        """(first, end): the absolute samples [first, end) the history holds once every run enqueued so far has finished."""
+        first, end = C.c_uint64(0), C.c_uint64(0)
+        self._chk(self.L.abg_history_range(self.h, dev, C.byref(first), C.byref(end)))
+        return int(first.value), int(end.value)
+
+    def history_raw(self, dev: int, first: int, n: int) -> np.ndarray:
+        """Samples [first, first + n) exactly as pushed: the ring dtype (uint8, int8, int16 or float32), I and Q
+        interleaved, 2 * n items."""
+        dt = {1: np.uint8, 2: np.int8, 3: np.int16, 4: np.float32}[self.cfg.devices[dev].sfmt] if 0 <= dev < len(self.cfg.devices) else np.uint8
+        out = np.empty(2 * max(int(n), 0), dt)
+        self._chk(self.L.abg_history_raw(self.h, dev, int(first), int(n), _ptr(out)))
+        return out
+
+    def history_subband(self, dev: int, offset_hz: float, decim: int, coeffs, first_m: int, n_out: int) -> np.ndarray:
+        """y[m] of the sub-band definition for m in [first_m, first_m + n_out), computed from the history: complex64[n_out],
+        bitwise what a live output of the same settings computes once all its taps follow its start."""
+        h = np.ascontiguousarray(coeffs, dtype=np.float32)
+        out = np.empty(2 * max(int(n_out), 0), np.float32)
+        self._chk(self.L.abg_history_subband(self.h, dev, float(offset_hz), int(decim), h.size, _ptr(h), int(first_m), int(n_out),
+                                             _ptr(out)))
+        return out.view(np.complex64)
+
+    def history_time(self) -> Tuple[float, float]:
+        """(append ms of the most recent run, kernel ms of the most recent history_subband), from CUDA events on the K1
+        stream; 0 where there was none."""
+        ms = (C.c_float * 2)()
+        self._chk(self.L.abg_debug_history_time(self.h, ms))
+        return float(ms[0]), float(ms[1])
 
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
@@ -861,3 +905,26 @@ def group_transmissions(bursts, cfg: Config, dev: int, max_bin_gap: int = 1, cen
                         monitored=any(lo <= c <= hi for c in chan_bins)))
     out.sort(key=lambda t: (t["first_frame"], t["freq_hz"]))
     return out
+
+
+def transmission_capture(tx: dict, cfg: Config, dev: int, history_range: Tuple[int, int], decim: int, n_coeffs: int,
+                         pad_s: float = 0.0) -> Tuple[float, int, int]:
+    """The Engine.history_subband window of one transmission (a group_transmissions dict of device dev): returns
+    (offset_hz, first_m, n_out).  offset_hz is tx["freq_hz"] from the device's centre frequency.  The window covers the
+    transmission's samples [first_frame * hop, last_frame * hop + fft_size), widened by pad_s seconds on each side, as the
+    outputs m with m * decim inside it, clipped so that every tap lies in history_range = (first, end):
+    m * decim - (n_coeffs - 1) >= first and m * decim < end.  Raises ValueError if no output is left."""
+    d = cfg.devices[dev]
+    hop, D, L = cfg.hop(dev), int(decim), int(n_coeffs)
+    if D < 1 or L < 1:
+        raise ValueError("transmission_capture: decim and n_coeffs must be >= 1")
+    pad = int(round(pad_s * d.sample_rate))
+    lo = max(int(tx["first_frame"]) * hop - pad, 0)
+    hi = int(tx["last_frame"]) * hop + cfg.fft_size + pad  # exclusive
+    first, end = history_range
+    m_lo = max(-(-lo // D), -(-(first + L - 1) // D))
+    m_hi = min(-(-hi // D), -(-end // D))  # exclusive: m * D < hi and m * D < end
+    if m_hi <= m_lo:
+        raise ValueError(f"transmission_capture: nothing of the transmission (samples [{lo}, {hi})) is left in the history "
+                         f"[{first}, {end}) with {L} taps at decimation {D}")
+    return float(tx["freq_hz"]) - float(d.centerfreq), m_lo, m_hi - m_lo

@@ -2,7 +2,7 @@
 process, plus the monitor kernel's own CUDA-event time and K1 / K2.  The card name and power limit are read in the same
 call.
 
-    python tools/monitor_overhead.py --monitor {spectrum,carrier,input_meter,subband,tone_meter,activity} [--workloads cfg2,cfg5] [--runs 40]
+    python tools/monitor_overhead.py --monitor {spectrum,carrier,input_meter,subband,tone_meter,activity,history} [--workloads cfg2,cfg5] [--runs 40]
                                      [--reps 3] [--out DIR]
 
 Legs:
@@ -15,6 +15,8 @@ Legs:
                the readings' transfer to host memory.
   activity     off, the default stride, stride 1; hang 1, min_span 1 and a uniform threshold of ACT_THR (|X|^2) for every
                bin.  Resident runs count pieces but store none, so these times leave out the records' transfer.
+  history      off, on for every device with a capacity of HIST_BATCHES batches (the append only; resident runs append
+               like streamed ones but leave the history empty).
 
 Prints one JSON line per workload (and writes it to DIR/<monitor>_overhead.jsonl with --out).  It uses only public
 lib.Engine methods, so ABG_LIB_PATH can point it at another build of the library."""
@@ -35,6 +37,7 @@ from airband_b200 import lib  # noqa: E402
 NB = 4  # batches per run, as bench.py's resident leg
 DECIM, NTAPS = 32, 255  # sub-band outputs
 ACT_THR = 1.0e4  # activity detector threshold, on the band spectrum's scale
+HIST_BATCHES = 8  # I/Q history capacity
 
 
 def raw_bytes_per_run(cfg):
@@ -94,6 +97,11 @@ MONITORS = {
         configure=activity_configure,
         time="activity_time", time_key="activity_ms", setting_key="stride",
         extra=lambda cfg: {"threshold": ACT_THR, "hang": 1, "min_span": 1}),
+    "history": dict(
+        legs=lambda cfg: {"off": 0, "on": HIST_BATCHES},
+        configure=lambda e, cfg, d, n: e.history_configure(d, n),
+        time="history_time", time_key="append_ms", setting_key="n_batches",
+        extra=lambda cfg: {"raw_bytes_read_and_written_per_run": raw_bytes_per_run(cfg)}),
 }
 
 
@@ -149,7 +157,8 @@ def main():
                     e.run_resident(NB)
                     t = e.last_run_times()
                     r["k1_ms"].append(t[0]); r["k2_ms"].append(t[1])
-                    r["kernel_ms"].append(kernel_time())
+                    t = kernel_time()
+                    r["kernel_ms"].append(t[0] if isinstance(t, tuple) else t)  # history_time: (append, capture)
         out = {"workload": name, "desc": desc, "card": card(), "batches_per_run": NB, "runs_per_leg": args.runs, "reps": args.reps,
                **mon["extra"](cfg)}
         for leg, setting in legs.items():
