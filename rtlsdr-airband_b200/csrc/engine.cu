@@ -154,17 +154,26 @@ bool plan_for(int n, Plan* p) {  // must match Plan<LOGN> in k1_fft.cu
     return false;
 }
 
+// Device memory.  A failed allocation leaves the buffer empty and clears the runtime's last error (an allocation error is
+// not sticky), so that the next launch check does not report it.
 template <typename T>
 struct DevBuf {
     T* p = nullptr;
     size_t n = 0;
     cudaError_t alloc(size_t count) {
-        n = count;
-        return cudaMalloc((void**)&p, std::max<size_t>(count, 1) * sizeof(T));
+        const cudaError_t er = cudaMalloc((void**)&p, std::max<size_t>(count, 1) * sizeof(T));
+        if (er == cudaSuccess) {
+            n = count;
+        } else {
+            cudaGetLastError();
+            p = nullptr;
+        }
+        return er;
     }
     void free() {
         if (p) cudaFree(p);
         p = nullptr;
+        n = 0;
     }
 };
 
@@ -184,27 +193,18 @@ struct MonitorQueue {
     int cap = 0, next = 0;
     std::deque<Entry> ready;
 
-    // false: out of page-locked memory.  Entries already queued survive (switching a monitor off and on keeps them).
-    bool alloc(int cap_, size_t entry_bytes_) {
-        if (ring) return true;
-        if (cudaHostAlloc((void**)&ring, (size_t)cap_ * entry_bytes_, cudaHostAllocMapped) != cudaSuccess) {
-            ring = nullptr;
+    // Room for entries of entry_bytes_ for an engine of max_batches_per_run.  A larger entry than the ring has moves the
+    // ring, entry by entry, so that what is queued survives (an entry size grows for sub-band outputs only); so do
+    // entries queued before the monitor was switched off and on again.  false: out of page-locked memory, the old ring
+    // is kept and the runtime's last error is cleared.
+    bool reserve(int max_batches_per_run, size_t entry_bytes_) {
+        if (ring && entry_bytes_ <= entry_bytes) return true;
+        const int cap_ = max_batches_per_run + 2;
+        unsigned char* grown = nullptr;
+        if (cudaHostAlloc((void**)&grown, (size_t)cap_ * entry_bytes_, cudaHostAllocMapped) != cudaSuccess) {
+            cudaGetLastError();
             return false;
         }
-        cap = cap_;
-        entry_bytes = entry_bytes_;
-        return true;
-    }
-    void release() {
-        if (ring) cudaFreeHost(ring);
-        ring = nullptr;
-    }
-    // Like alloc, for a monitor whose entry size can grow (sub-band outputs): a larger entry moves the ring, entry by
-    // entry, so that what is queued survives.  false: out of page-locked memory, the old ring is kept.
-    bool reserve(int cap_, size_t entry_bytes_) {
-        if (ring && entry_bytes_ <= entry_bytes) return true;
-        unsigned char* grown = nullptr;
-        if (cudaHostAlloc((void**)&grown, (size_t)cap_ * entry_bytes_, cudaHostAllocMapped) != cudaSuccess) return false;
         if (ring) {
             for (int i = 0; i < cap; i++) memcpy(grown + (size_t)i * entry_bytes_, ring + (size_t)i * entry_bytes, entry_bytes);
             cudaFreeHost(ring);
@@ -213,6 +213,10 @@ struct MonitorQueue {
         cap = cap_;
         entry_bytes = entry_bytes_;
         return true;
+    }
+    void release() {
+        if (ring) cudaFreeHost(ring);
+        ring = nullptr;
     }
     // Queue the n batches of run `run` whose first is batch number seq0; returns the ring entry of the first.
     int queue(int n, uint64_t seq0, uint64_t run, int32_t aux) {
@@ -226,19 +230,140 @@ struct MonitorQueue {
 
 constexpr int TL_RUNS = 8;  // runs whose timing events are kept
 
-// Host side of one batch monitor's launch: one kernel per run covers every device the monitor is on for.  The
-// sequence around it is shared (monitor_on, monitor_publish, monitor_launch, monitor_time); DESIGN.md §4, "Engine
-// plumbing", states its contract.
-template <typename Cfg, typename Run>
+// Host side of one batch monitor: its state per engine device, and its launch, one kernel per run that covers every
+// device the monitor is on for.  The sequence around it is shared (monitor_dev, monitor_configure, monitor_publish,
+// monitor_launch, monitor_time, monitor_fetch); DESIGN.md §4, "Engine plumbing", states its contract.  Dev is the
+// monitor's own per-device state: on() tells whether the launch covers the device, release() frees what it holds.
+template <typename Cfg, typename Run, typename Dev>
 struct MonitorLaunch {
     const char* name;        // in error messages
     bool reads_raw;          // reads raw[] after K1: records ev_raw, which abg_push's compaction waits for
+    bool after_k2;           // runs on stream B after K2 (it reads the audio), not on stream A after K1
+    std::vector<Dev> dev;    // [engine devices]; nothing is allocated for a device until it is first switched on
     std::vector<int> devs;   // covered devices in launch order (grid.y of the kernel)
     DevBuf<Cfg> cfg;         // [devs.size()], written when a configure call changes the list
     DevBuf<Run> run;         // room for every device, uploaded with every run
     std::vector<Run> h_run;  // [devs.size()]
     cudaEvent_t tl[TL_RUNS][2] = {};  // kernel start / end of the last TL_RUNS runs
     bool ran[TL_RUNS] = {};
+
+    MonitorLaunch(const char* name_, bool reads_raw_, bool after_k2_ = false) : name(name_), reads_raw(reads_raw_), after_k2(after_k2_) {}
+    void release() {
+        for (auto& d : dev) d.release();
+        cfg.free();
+        run.free();
+        for (auto& row : tl)
+            for (auto& ev : row)
+                if (ev) cudaEventDestroy(ev);
+    }
+};
+
+// band spectrum (abg_spectrum_configure)
+struct SpecDev {
+    int stride = 0, n_sel = 0, chunks = 0;
+    DevBuf<unsigned char> work;  // chunk sums float[nbmax][chunks][N], then the batch counters int32[nbmax]
+    MonitorQueue q;              // finished spectra float[N] per entry
+    bool on() const { return stride > 0; }
+    MonitorQueue& queue(int) { return q; }
+    void release() { work.free(); q.release(); }
+};
+// carrier frequency meter (abg_carrier_configure)
+struct CarDev {
+    bool enabled = false;
+    MonitorQueue q;  // lag1 float[C][2], then energy float[C] per entry
+    bool on() const { return enabled; }
+    MonitorQueue& queue(int) { return q; }
+    void release() { q.release(); }
+};
+// input level meter (abg_input_meter_configure)
+struct InmDev {
+    bool enabled = false;
+    int chunks = 0;
+    DevBuf<unsigned char> work;  // histograms uint32[nbmax][2][256], counters int32[nbmax], chunk sums int64[nbmax][chunks][ABG_INM_PARTIAL]; kept once allocated
+    MonitorQueue q;              // abg_input_levels per entry
+    bool on() const { return enabled; }
+    MonitorQueue& queue(int) { return q; }
+    void release() { work.free(); q.release(); }
+};
+// sub-band I/Q outputs (abg_subband_configure)
+struct SbDev {
+    struct Output {
+        bool on = false;
+        bool restart = false;        // the next streamed run starts the output's input at its first batch
+        int decim = 0, n_coeffs = 0;
+        uint32_t delta = 0;
+        long long start = 0;         // absolute sample index of the output's first input sample
+        DevBuf<float2> coef;         // h[j] * exp(+2 pi i delta j / 2^32); kept once allocated
+        MonitorQueue q;              // cf32 [ceil(n / decim)] per entry, Entry.aux = decim
+    } out[ABG_SUBBAND_MAX];
+    int hist = 0;                    // L_max - 1 over the outputs switched on: samples abg_push's compaction keeps before `consumed`
+    bool on() const { return std::any_of(std::begin(out), std::end(out), [](const Output& o) { return o.on; }); }
+    MonitorQueue& queue(int k) { return out[k].q; }
+    void release() {
+        for (auto& o : out) {
+            o.coef.free();
+            o.q.release();
+        }
+    }
+};
+struct SubbandLaunch : MonitorLaunch<SbCfg, SbRun, SbDev> {
+    using MonitorLaunch::MonitorLaunch;
+    int max_hist = 0;  // largest SbDev::hist of devs
+};
+// CTCSS tone meter (abg_tone_meter_configure)
+struct TmDev {
+    bool enabled = false;
+    MonitorQueue q;  // S float[C][K][2], E float[C], active int32[C] per entry (room for ABG_TONE_MAX), Entry.aux = K
+    bool on() const { return enabled; }
+    MonitorQueue& queue(int) { return q; }
+    void release() { q.release(); }
+};
+struct ToneMeterLaunch : MonitorLaunch<TmCfg, TmRun, TmDev> {
+    using MonitorLaunch::MonitorLaunch;
+    // the engine-wide tone list and, once the meter is first switched on, its [B][cols] table
+    std::vector<float> freqs{std::begin(kStandardTones), std::end(kStandardTones)};
+    std::vector<uint32_t> delta;
+    DevBuf<float> table;
+    int cols = 0;
+    DevBuf<int32_t> chan_dev;  // metered channel -> index into devs
+    int n_chan = 0;
+    void release() {
+        MonitorLaunch::release();
+        table.free();
+        chan_dev.free();
+    }
+};
+// band activity detector (abg_activity_configure)
+struct ActDev {
+    int stride = 0, hang = 0, min_span = 0, n_sel = 0;
+    DevBuf<float> thr;  // [N] thresholds; kept once allocated
+    MonitorQueue q;     // head int32[4] {n_total, stride, hang, min_span}, then abg_burst[ABG_ACTIVITY_MAX_RECORDS]
+    bool on() const { return stride > 0; }
+    MonitorQueue& queue(int) { return q; }
+    void release() { thr.free(); q.release(); }
+};
+// I/Q history (abg_history_configure); its ring is freed when it is switched off
+struct HiDev {
+    int batches = 0;                       // capacity in batches, 0 = off
+    DevBuf<unsigned char> ring;            // stream byte b at b mod ring.n; ring.n = cap * bpc rounded up to a multiple of 16
+    unsigned long long cap = 0;            // capacity in samples
+    unsigned long long first = 0, end = 0;  // samples [first, end) the ring holds once every enqueued run has finished
+    bool on() const { return ring.p != nullptr; }
+    void release() { ring.free(); }
+};
+struct HistoryLaunch : MonitorLaunch<HiCfg, HiRun, HiDev> {
+    using MonitorLaunch::MonitorLaunch;
+    // captures: coefficient and output scratch (allocated by the first capture) and the last capture's kernel time
+    DevBuf<float2> coef, out;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    float capture_ms = 0.0f;
+    void release() {
+        MonitorLaunch::release();
+        coef.free();
+        out.free();
+        for (auto& x : ev)
+            if (x) cudaEventDestroy(x);
+    }
 };
 
 struct Device {
@@ -259,43 +384,7 @@ struct Device {
     std::deque<std::pair<int, int>> ready;  // (slot, batch-in-run)
     uint64_t batch_seq = 0;  // batches of the pushed stream enqueued since abg_create
     uint64_t audio_seq = 0;  // batches queued for abg_fetch_batch since abg_create, pushed and injected
-    // band spectrum monitor (abg_spectrum_configure); nothing is allocated until it is first switched on
-    int spec_stride = 0, spec_n_sel = 0, spec_chunks = 0;
-    void* spec_work = nullptr;   // device: chunk sums float[nbmax][spec_chunks][N], then the batch counters int32[nbmax]
-    MonitorQueue spec_q;         // finished spectra float[N] per entry
-    // carrier frequency meter (abg_carrier_configure); nothing is allocated until it is first switched on
-    bool car_on = false;
-    MonitorQueue car_q;          // lag1 float[C][2], then energy float[C] per entry
-    // input level meter (abg_input_meter_configure); nothing is allocated until it is first switched on
-    bool inm_on = false;
-    int inm_chunks = 0;
-    void* inm_work = nullptr;    // device: histograms uint32[nbmax][2][256], counters int32[nbmax], chunk sums int64[nbmax][inm_chunks][ABG_INM_PARTIAL]; kept once allocated
-    MonitorQueue inm_q;          // abg_input_levels per entry
-    // sub-band I/Q outputs (abg_subband_configure); nothing is allocated until one is first switched on
-    struct Subband {
-        bool on = false;
-        bool restart = false;        // the next streamed run starts the output's input at its first batch
-        int decim = 0, n_coeffs = 0, coef_cap = 0;
-        uint32_t delta = 0;
-        long long start = 0;         // absolute sample index of the output's first input sample
-        float2* coef = nullptr;      // device [coef_cap]: h[j] * exp(+2 pi i delta j / 2^32); kept once allocated
-        MonitorQueue q;              // cf32 [ceil(n / decim)] per entry, Entry.aux = decim
-    } sb[ABG_SUBBAND_MAX];
-    int sb_hist = 0;                 // L_max - 1 over the outputs switched on: samples compaction keeps before `consumed`
-    size_t dropped = 0;              // stream bytes compaction has dropped: raw[cur][0] is byte `dropped` of the stream
-    // CTCSS tone meter (abg_tone_meter_configure); nothing is allocated until it is first switched on
-    bool tm_on = false;
-    MonitorQueue tm_q;               // S float[C][K][2], E float[C], active int32[C] per entry (room for ABG_TONE_MAX), Entry.aux = K
-    // band activity detector (abg_activity_configure); nothing is allocated until it is first switched on
-    int act_stride = 0, act_hang = 0, act_min_span = 0, act_n_sel = 0;
-    float* act_thr = nullptr;        // device [N] thresholds; kept once allocated
-    MonitorQueue act_q;              // head int32[4] {n_total, stride, hang, min_span}, then abg_burst[ABG_ACTIVITY_MAX_RECORDS]
-    // I/Q history (abg_history_configure); nothing is allocated until it is first switched on, and it is freed when off
-    int hi_batches = 0;                    // capacity in batches, 0 = off
-    unsigned char* hi_ring = nullptr;      // device [hi_ring_bytes]: stream byte b at b mod hi_ring_bytes
-    unsigned long long hi_ring_bytes = 0;  // hi_cap * bpc rounded up to a multiple of 16
-    unsigned long long hi_cap = 0;         // capacity in samples
-    unsigned long long hi_first = 0, hi_end = 0;  // samples [first, end) the ring holds once every enqueued run has finished
+    size_t dropped = 0;      // stream bytes compaction has dropped: raw[cur][0] is byte `dropped` of the stream
 };
 
 // ---- scan mode: per-frequency freq_t sets (rtl_airband.h:223-233,250-252) ------------------------------------------------
@@ -432,25 +521,17 @@ struct abg_engine {
     std::vector<int32_t> h_bins;
     // batch monitors: the first four, the activity detector and the I/Q history's append are launched in this order on
     // stream A after K1, the tone meter on stream B after K2
-    MonitorLaunch<SpecCfg, SpecRun> spectrum{"spectrum", true};
-    MonitorLaunch<CarCfg, CarRun> carrier{"carrier meter", false};
-    MonitorLaunch<InmCfg, InmRun> input_meter{"input meter", true};
-    MonitorLaunch<SbCfg, SbRun> subband{"sub-band", true};
-    MonitorLaunch<TmCfg, TmRun> tone_meter{"tone meter", false};
-    MonitorLaunch<ActCfg, ActRun> activity{"activity detector", true};
-    MonitorLaunch<HiCfg, HiRun> history{"I/Q history", true};  // the append, last on stream A
-    // I/Q history captures: coefficient and output scratch (allocated by the first capture) and the last capture's kernel time
-    DevBuf<float2> hi_coef, hi_out;
-    cudaEvent_t hi_ev[2] = {nullptr, nullptr};
-    float hi_capture_ms = 0.0f;
-    // tone meter tables: the engine-wide tone list and, once the meter is first switched on, its [B][tm_cols] table
-    std::vector<float> tm_freqs{std::begin(kStandardTones), std::end(kStandardTones)};
-    std::vector<uint32_t> tm_delta;
-    DevBuf<float> tm_table;
-    int tm_cols = 0;
-    DevBuf<int32_t> tm_chan_dev;  // metered channel -> index into tone_meter.devs
-    int tm_n_chan = 0;
-    int sb_max_hist = 0;  // largest Device::sb_hist of subband.devs
+    MonitorLaunch<SpecCfg, SpecRun, SpecDev> spectrum{"spectrum", true};
+    MonitorLaunch<CarCfg, CarRun, CarDev> carrier{"carrier meter", false};
+    MonitorLaunch<InmCfg, InmRun, InmDev> input_meter{"input meter", true};
+    SubbandLaunch subband{"sub-band", true};
+    ToneMeterLaunch tone_meter{"tone meter", false, true};
+    MonitorLaunch<ActCfg, ActRun, ActDev> activity{"activity detector", true};
+    HistoryLaunch history{"I/Q history", true};  // the append, last on stream A
+    template <typename F>
+    void each_monitor(F&& f) {
+        f(spectrum); f(carrier); f(input_meter); f(subband); f(tone_meter); f(activity); f(history);
+    }
     // after the last monitor that read raw[] in the latest run of each parity that launched one; created when the first
     // such monitor is switched on
     cudaEvent_t ev_raw[2] = {nullptr, nullptr};
@@ -478,9 +559,29 @@ struct abg_engine {
 
 namespace {
 
-// Switching a monitor on for its first device creates its timing events, and ev_raw if it reads raw[].
-template <typename Cfg, typename Run>
-int monitor_on(abg_engine* e, MonitorLaunch<Cfg, Run>& m) {
+// The stream a monitor's kernel runs on: B after K2 for a monitor of the audio, A after K1 for the others.
+template <typename Cfg, typename Run, typename Dev>
+cudaStream_t monitor_stream(const abg_engine* e, const MonitorLaunch<Cfg, Run, Dev>& m) {
+    return m.after_k2 ? e->stream_b : e->stream;
+}
+
+// Device `dev`'s state in monitor m; null, after an ABG_ERANGE failure naming the entry point fn, for a device the engine
+// does not have.
+template <typename Cfg, typename Run, typename Dev>
+Dev* monitor_dev(abg_engine* e, MonitorLaunch<Cfg, Run, Dev>& m, int dev, const char* fn) {
+    if (dev >= 0 && dev < (int)m.dev.size()) return &m.dev[dev];
+    fail(ABG_ERANGE, "%s: device %d out of range", fn, dev);
+    return nullptr;
+}
+
+// Start of a configure call that changes something, after its own checks: wait until no enqueued kernel of the monitor
+// can still read its tables and buffers, then, if the call switches a device on, create the monitor's timing events
+// and, if it reads raw[], ev_raw (each once).
+template <typename Cfg, typename Run, typename Dev>
+int monitor_configure(abg_engine* e, MonitorLaunch<Cfg, Run, Dev>& m, bool on) {
+    cudaSetDevice(e->cuda_dev);
+    CU(cudaStreamSynchronize(monitor_stream(e, m)));
+    if (!on) return ABG_OK;
     if (!m.tl[0][0])
         for (auto& row : m.tl)
             for (auto& ev : row) CU(cudaEventCreate(&ev));
@@ -489,9 +590,21 @@ int monitor_on(abg_engine* e, MonitorLaunch<Cfg, Run>& m) {
     return ABG_OK;
 }
 
-// Install the device list and static table a configure call built.  With no device left nothing is allocated.
-template <typename Cfg, typename Run>
-int monitor_publish(abg_engine* e, MonitorLaunch<Cfg, Run>& m, const std::vector<int>& devs, const std::vector<Cfg>& cfgs) {
+// End of a configure call: rebuild the launch's device list and static table from the per-device state, in device
+// order.  `fill(device, state, cfg)` writes the table entry of each device the monitor is on for and returns ABG_OK or
+// an error.  With no device left nothing is allocated.
+template <typename Cfg, typename Run, typename Dev, typename Fill>
+int monitor_publish(abg_engine* e, MonitorLaunch<Cfg, Run, Dev>& m, Fill&& fill) {
+    std::vector<int> devs;
+    std::vector<Cfg> cfgs;
+    for (int i = 0; i < (int)m.dev.size(); i++) {
+        if (!m.dev[i].on()) continue;
+        Cfg c{};
+        const int rc = fill(e->dev[i], m.dev[i], c);
+        if (rc != ABG_OK) return rc;
+        devs.push_back(i);
+        cfgs.push_back(c);
+    }
     m.devs = devs;
     m.cfg.free();
     m.h_run.assign(devs.size(), Run{});
@@ -504,12 +617,23 @@ int monitor_publish(abg_engine* e, MonitorLaunch<Cfg, Run>& m, const std::vector
     return ABG_OK;
 }
 
-// One run of a monitor on stream st (A after K1, or B after K2), after its h_run records are filled: their upload, then
+// Per-run records of a monitor: `each(run record, monitor state, device, n)` for every device it covers, n the device's
+// batches in this run.
+template <typename Cfg, typename Run, typename Dev, typename Each>
+void monitor_runs(abg_engine* e, MonitorLaunch<Cfg, Run, Dev>& m, const std::vector<int>& nb, Each&& each) {
+    for (size_t k = 0; k < m.devs.size(); k++) {
+        const int i = m.devs[k];
+        each(m.h_run[k], m.dev[i], e->dev[i], nb[i]);
+    }
+}
+
+// One run of a monitor on its stream, after its h_run records are filled: their upload, then
 // `kernel(n_devices, max_items, stream)` between the timing events, then ev_raw if it reads raw[].  Nothing when max_items
 // is 0.
-template <typename Cfg, typename Run, typename Kernel>
-int monitor_launch(abg_engine* e, MonitorLaunch<Cfg, Run>& m, int max_items, cudaStream_t st, Kernel&& kernel) {
+template <typename Cfg, typename Run, typename Dev, typename Kernel>
+int monitor_launch(abg_engine* e, MonitorLaunch<Cfg, Run, Dev>& m, int max_items, Kernel&& kernel) {
     if (max_items <= 0) return ABG_OK;
+    const cudaStream_t st = monitor_stream(e, m);
     const int t = (int)(e->run_index % TL_RUNS);
     const int nl = upload_small(m.run.p, m.h_run.data(), sizeof(Run) * m.devs.size(), st);
     if (nl < 0) return fail(ABG_ECUDA, "%s parameter upload failed: %s", m.name, cudaGetErrorString(cudaGetLastError()));
@@ -525,8 +649,8 @@ int monitor_launch(abg_engine* e, MonitorLaunch<Cfg, Run>& m, int max_items, cud
 }
 
 // ms of the monitor's kernel in the most recent run; 0 if that run did not launch it.  `fn` names the entry point.
-template <typename Cfg, typename Run>
-int monitor_time(abg_engine* e, const MonitorLaunch<Cfg, Run>& m, float* ms, const char* fn) {
+template <typename Cfg, typename Run, typename Dev>
+int monitor_time(abg_engine* e, const MonitorLaunch<Cfg, Run, Dev>& m, float* ms, const char* fn) {
     if (!ms) return fail(ABG_EINVAL, "%s: null argument", fn);
     *ms = 0.0f;
     if (e->run_index == 0 || !m.ran[(e->run_index - 1) % TL_RUNS]) return ABG_OK;
@@ -537,10 +661,15 @@ int monitor_time(abg_engine* e, const MonitorLaunch<Cfg, Run>& m, float* ms, con
     return ABG_OK;
 }
 
-// Pop the oldest entry of one of monitor m's queues once m's kernel of the entry's run has finished: returns 1 and the
-// entry's ring bytes in *data, 0 if the queue is empty, < 0 on error.
-template <typename Cfg, typename Run>
-int monitor_pop(abg_engine* e, MonitorQueue& q, const MonitorLaunch<Cfg, Run>& m, const unsigned char** data, MonitorQueue::Entry* got) {
+// Start of a fetch: pop the oldest entry of device dev's queue k once m's kernel of the entry's run has finished.  Returns
+// 1 and the entry's ring bytes in *data, 0 if the queue is empty, < 0 on error (ABG_ERANGE for a device the engine does not
+// have, naming the entry point fn).
+template <typename Cfg, typename Run, typename Dev>
+int monitor_fetch(abg_engine* e, MonitorLaunch<Cfg, Run, Dev>& m, int dev, int k, const char* fn, const unsigned char** data,
+                  MonitorQueue::Entry* got) {
+    Dev* d = monitor_dev(e, m, dev, fn);
+    if (!d) return ABG_ERANGE;
+    MonitorQueue& q = d->queue(k);
     if (q.ready.empty()) return 0;
     *got = q.ready.front();
     cudaSetDevice(e->cuda_dev);
@@ -548,15 +677,6 @@ int monitor_pop(abg_engine* e, MonitorQueue& q, const MonitorLaunch<Cfg, Run>& m
     *data = q.ring + (size_t)got->pos * q.entry_bytes;
     q.ready.pop_front();  // the bytes stay put until a later run is enqueued
     return 1;
-}
-
-template <typename Cfg, typename Run>
-void monitor_free(MonitorLaunch<Cfg, Run>& m) {
-    m.cfg.free();
-    m.run.free();
-    for (auto& row : m.tl)
-        for (auto& ev : row)
-            if (ev) cudaEventDestroy(ev);
 }
 
 void engine_free(abg_engine* e) {
@@ -569,33 +689,8 @@ void engine_free(abg_engine* e) {
             if (d.raw[i]) cudaFree(d.raw[i]);
         if (d.res) cudaFree(d.res);
         if (d.spec) cudaFree(d.spec);
-        if (d.spec_work) cudaFree(d.spec_work);
-        if (d.inm_work) cudaFree(d.inm_work);
-        d.spec_q.release();
-        d.car_q.release();
-        d.inm_q.release();
-        d.tm_q.release();
-        if (d.act_thr) cudaFree(d.act_thr);
-        d.act_q.release();
-        if (d.hi_ring) cudaFree(d.hi_ring);
-        for (auto& so : d.sb) {
-            if (so.coef) cudaFree(so.coef);
-            so.q.release();
-        }
     }
-    monitor_free(e->spectrum);
-    monitor_free(e->carrier);
-    monitor_free(e->input_meter);
-    monitor_free(e->subband);
-    monitor_free(e->tone_meter);
-    monitor_free(e->activity);
-    monitor_free(e->history);
-    e->hi_coef.free();
-    e->hi_out.free();
-    for (auto& ev : e->hi_ev)
-        if (ev) cudaEventDestroy(ev);
-    e->tm_table.free();
-    e->tm_chan_dev.free();
+    e->each_monitor([](auto& m) { m.release(); });
     for (auto& g : e->groups) {
         g.wsc.free();
         g.tc_btab.free(); g.tc_sq.free(); g.tc_tab_of_dev.free();
@@ -782,6 +877,7 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
 
     // ---- devices, channel index space ------------------------------------------------------------------------
     e->dev.resize(cfg->n_devices);
+    e->each_monitor([&](auto& m) { m.dev.resize(cfg->n_devices); });
     int G = 0;
     for (int i = 0; i < cfg->n_devices; i++) {
         const abg_device_cfg& dc = cfg->devices[i];
@@ -1125,21 +1221,21 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     // outputs, the activity detector; K2 does not wait for them past ev_k1).  Injected batches have no frames and launch
     // none. ----
     const int t = (int)(ri % TL_RUNS);
-    e->spectrum.ran[t] = e->carrier.ran[t] = e->input_meter.ran[t] = e->subband.ran[t] = e->tone_meter.ran[t] = false;
-    e->activity.ran[t] = e->history.ran[t] = false;
+    e->each_monitor([t](auto& m) { m.ran[t] = false; });
+    // n_batches and ring_pos0 of a monitor with one queue per device: resident runs queue nothing
+    auto queue_run = [&](auto& r, MonitorQueue& q, int n, uint64_t seq0, int32_t aux) {
+        r.n_batches = n;
+        r.ring_pos0 = queue_outputs && n > 0 ? q.queue(n, seq0, ri, aux) : -1;
+    };
     if (!skip_k1) {
         int max_items = 0;
-        for (size_t m = 0; m < e->spectrum.devs.size(); m++) {
-            Device& d = e->dev[e->spectrum.devs[m]];
-            const int n = nb[e->spectrum.devs[m]];
-            SpecRun& r = e->spectrum.h_run[m];
+        monitor_runs(e, e->spectrum, nb, [&](SpecRun& r, SpecDev& s, Device& d, int n) {
             r.raw = resident ? d.res : d.raw[d.cur];
             r.first_byte = run_first_byte(d, resident);
-            r.n_batches = n;
-            r.ring_pos0 = queue_outputs && n > 0 ? d.spec_q.queue(n, d.batch_seq, ri, d.spec_n_sel) : -1;
-            max_items = std::max(max_items, n * d.spec_chunks);
-        }
-        int rc = monitor_launch(e, e->spectrum, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+            queue_run(r, s.q, n, d.batch_seq, s.n_sel);
+            max_items = std::max(max_items, n * s.chunks);
+        });
+        int rc = monitor_launch(e, e->spectrum, max_items, [&](int n_devices, int items, cudaStream_t s) {
             SpecArgs A{};
             A.cfg = e->spectrum.cfg.p; A.run = e->spectrum.run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
             return abg_launch_spectrum(N, A, n_devices, items, s);
@@ -1147,48 +1243,37 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
         if (rc != ABG_OK) return rc;
         // the carrier meter reads iqin[cur], which the next K1 to write it, two runs later, queues behind on this stream
         max_items = 0;
-        for (size_t m = 0; m < e->carrier.devs.size(); m++) {
-            Device& d = e->dev[e->carrier.devs[m]];
-            const int n = nb[e->carrier.devs[m]];
-            CarRun& r = e->carrier.h_run[m];
-            r.n_batches = n;
-            r.ring_pos0 = queue_outputs && n > 0 ? d.car_q.queue(n, d.batch_seq, ri, 0) : -1;
+        monitor_runs(e, e->carrier, nb, [&](CarRun& r, CarDev& s, Device& d, int n) {
+            queue_run(r, s.q, n, d.batch_seq, 0);
             max_items = std::max(max_items, n * abg_carrier_items(d.C));
-        }
-        rc = monitor_launch(e, e->carrier, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+        });
+        rc = monitor_launch(e, e->carrier, max_items, [&](int n_devices, int items, cudaStream_t s) {
             CarArgs A{};
             A.cfg = e->carrier.cfg.p; A.run = e->carrier.run.p; A.iqin = e->iqin[cur].p; A.Gp = e->Gp; A.wave_batch = B;
             return abg_launch_carrier(A, n_devices, items, s);
         });
         if (rc != ABG_OK) return rc;
         max_items = 0;
-        for (size_t m = 0; m < e->input_meter.devs.size(); m++) {
-            Device& d = e->dev[e->input_meter.devs[m]];
-            const int n = nb[e->input_meter.devs[m]];
-            InmRun& r = e->input_meter.h_run[m];
+        monitor_runs(e, e->input_meter, nb, [&](InmRun& r, InmDev& s, Device& d, int n) {
             r.raw = resident ? d.res : d.raw[d.cur];
             r.first_byte = run_first_byte(d, resident);
-            r.n_batches = n;
-            r.ring_pos0 = queue_outputs && n > 0 ? d.inm_q.queue(n, d.batch_seq, ri, 0) : -1;
-            max_items = std::max(max_items, n * d.inm_chunks);
-        }
-        rc = monitor_launch(e, e->input_meter, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+            queue_run(r, s.q, n, d.batch_seq, 0);
+            max_items = std::max(max_items, n * s.chunks);
+        });
+        rc = monitor_launch(e, e->input_meter, max_items, [&](int n_devices, int items, cudaStream_t s) {
             InmArgs A{};
             A.cfg = e->input_meter.cfg.p; A.run = e->input_meter.run.p; A.wave_batch = B;
             return abg_launch_input_meter(A, n_devices, items, s);
         });
         if (rc != ABG_OK) return rc;
         max_items = 0;
-        for (size_t m = 0; m < e->subband.devs.size(); m++) {
-            Device& d = e->dev[e->subband.devs[m]];
-            const int n = nb[e->subband.devs[m]];
-            SbRun& r = e->subband.h_run[m];
+        monitor_runs(e, e->subband, nb, [&](SbRun& r, SbDev& s, Device& d, int n) {
             r.raw = resident ? d.res : d.raw[d.cur];
             r.base = resident ? 0 : (long long)(d.dropped / d.bpc);
             r.s0 = r.base + (long long)(run_first_byte(d, resident) / d.bpc);
             r.n_batches = n;
             int o = 0;
-            for (auto& so : d.sb) {
+            for (auto& so : s.out) {
                 if (!so.on) continue;
                 if (!resident && n > 0 && so.restart) {
                     so.start = r.s0;
@@ -1199,26 +1284,22 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
                 o++;
             }
             max_items = std::max(max_items, n * abg_subband_chunks(B * d.hop));
-        }
-        rc = monitor_launch(e, e->subband, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+        });
+        rc = monitor_launch(e, e->subband, max_items, [&](int n_devices, int items, cudaStream_t s) {
             SbArgs A{};
             A.cfg = e->subband.cfg.p; A.run = e->subband.run.p;
-            return abg_launch_subband(A, n_devices, items, e->sb_max_hist, s);
+            return abg_launch_subband(A, n_devices, items, e->subband.max_hist, s);
         });
         if (rc != ABG_OK) return rc;
         max_items = 0;
-        for (size_t m = 0; m < e->activity.devs.size(); m++) {
-            Device& d = e->dev[e->activity.devs[m]];
-            const int n = nb[e->activity.devs[m]];
-            ActRun& r = e->activity.h_run[m];
+        monitor_runs(e, e->activity, nb, [&](ActRun& r, ActDev& s, Device& d, int n) {
             r.raw = resident ? d.res : d.raw[d.cur];
             r.first_byte = run_first_byte(d, resident);
             r.first_frame = (unsigned long long)ABG_AGC_EXTRA + d.batch_seq * (unsigned long long)B;
-            r.n_batches = n;
-            r.ring_pos0 = queue_outputs && n > 0 ? d.act_q.queue(n, d.batch_seq, ri, 0) : -1;
+            queue_run(r, s.q, n, d.batch_seq, 0);
             max_items = std::max(max_items, n);
-        }
-        rc = monitor_launch(e, e->activity, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+        });
+        rc = monitor_launch(e, e->activity, max_items, [&](int n_devices, int items, cudaStream_t s) {
             ActArgs A{};
             A.cfg = e->activity.cfg.p; A.run = e->activity.run.p; A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
             return abg_launch_activity(N, A, n_devices, items, s);
@@ -1227,30 +1308,27 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
         // the I/Q history's append: the run's samples [s0, s0 + n) of every device with the history on, at most the last
         // ring-full of them.  Resident runs append from the replay buffer at its own offsets and leave the history empty.
         unsigned long long max_bytes = 0;
-        for (size_t m = 0; m < e->history.devs.size(); m++) {
-            Device& d = e->dev[e->history.devs[m]];
-            const int n = nb[e->history.devs[m]];
-            HiRun& r = e->history.h_run[m];
+        monitor_runs(e, e->history, nb, [&](HiRun& r, HiDev& h, Device& d, int n) {
             const unsigned long long first_byte = run_first_byte(d, resident);
             const unsigned long long stream_byte = (resident ? 0ull : (unsigned long long)d.dropped) + first_byte;
-            const unsigned long long bytes = (unsigned long long)n * B * d.hop_bytes, R = d.hi_ring_bytes;
+            const unsigned long long bytes = (unsigned long long)n * B * d.hop_bytes, R = h.ring.n;
             const unsigned long long skip = bytes > R ? bytes - R : 0;
             r.src = (resident ? d.res : d.raw[d.cur]) + first_byte + skip;
             r.dst = (stream_byte + skip) % R;
             r.n_bytes = bytes - skip;
             max_bytes = std::max(max_bytes, r.n_bytes);
-            if (n == 0) continue;
+            if (n == 0) return;
             if (resident) {
-                d.hi_first = d.hi_end = 0;
-                continue;
+                h.first = h.end = 0;
+                return;
             }
             const unsigned long long s0 = stream_byte / d.bpc;
-            if (d.hi_first == d.hi_end || s0 != d.hi_end) d.hi_first = s0;
-            d.hi_end = s0 + (unsigned long long)n * B * d.hop;
-            if (d.hi_end - d.hi_first > d.hi_cap) d.hi_first = d.hi_end - d.hi_cap;
-        }
+            if (h.first == h.end || s0 != h.end) h.first = s0;
+            h.end = s0 + (unsigned long long)n * B * d.hop;
+            if (h.end - h.first > h.cap) h.first = h.end - h.cap;
+        });
         max_items = max_bytes > 0 ? abg_history_blocks(max_bytes, (int)e->history.devs.size(), e->sm_count) : 0;
-        rc = monitor_launch(e, e->history, max_items, sa, [&](int n_devices, int items, cudaStream_t s) {
+        rc = monitor_launch(e, e->history, max_items, [&](int n_devices, int items, cudaStream_t s) {
             HiArgs A{};
             A.cfg = e->history.cfg.p; A.run = e->history.run.p;
             return abg_launch_history_append(A, n_devices, items, s);
@@ -1291,22 +1369,19 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     // ---- tone meter (stream B after K2 and the mixers, pushed and injected batches alike): it reads wout[0, nb*B) before
     // the tail copy below overwrites [0, AGC_EXTRA), and the next run's K2 queues behind it on this stream ----
     {
-        const int K = (int)e->tm_freqs.size();
+        ToneMeterLaunch& m = e->tone_meter;
+        const int K = (int)m.freqs.size();
         int max_items = 0;
-        for (size_t m = 0; m < e->tone_meter.devs.size(); m++) {
-            Device& d = e->dev[e->tone_meter.devs[m]];
-            const int n = nb[e->tone_meter.devs[m]];
-            TmRun& r = e->tone_meter.h_run[m];
+        monitor_runs(e, m, nb, [&](TmRun& r, TmDev& s, Device& d, int n) {
             r.seq0 = d.audio_seq;
-            r.n_batches = n;
-            r.ring_pos0 = queue_outputs && n > 0 ? d.tm_q.queue(n, d.audio_seq, ri, K) : -1;
+            queue_run(r, s.q, n, d.audio_seq, K);
             max_items = std::max(max_items, n);
-        }
-        const int rc = monitor_launch(e, e->tone_meter, max_items, sb, [&](int, int items, cudaStream_t s) {
+        });
+        const int rc = monitor_launch(e, m, max_items, [&](int, int items, cudaStream_t s) {
             TmArgs A{};
-            A.cfg = e->tone_meter.cfg.p; A.run = e->tone_meter.run.p; A.chan_dev = e->tm_chan_dev.p; A.table = e->tm_table.p;
-            A.wout = e->wout.p; A.P = e->P; A.wave_batch = B; A.K = K; A.n_cols = e->tm_cols; A.n_chan = e->tm_n_chan;
-            for (int k = 0; k < K; k++) A.delta[k] = e->tm_delta[k];
+            A.cfg = m.cfg.p; A.run = m.run.p; A.chan_dev = m.chan_dev.p; A.table = m.table.p;
+            A.wout = e->wout.p; A.P = e->P; A.wave_batch = B; A.K = K; A.n_cols = m.cols; A.n_chan = m.n_chan;
+            for (int k = 0; k < K; k++) A.delta[k] = m.delta[k];
             return abg_launch_tone_meter(A, items, s);
         });
         if (rc != ABG_OK) return rc;
@@ -1420,7 +1495,7 @@ int abg_push(abg_engine* e, int dev, const void* iq, size_t nbytes) {
         // compact: move the unconsumed tail to the front of the other buffer.  Ingest runs on its own stream so that
         // host->device copies overlap K1; the other buffer may still be read by the most recent K1, so wait for it.
         // keep the copy 16-byte aligned on both sides; with a sub-band output on, keep its filter's history too
-        const size_t hist = (size_t)d.sb_hist * d.bpc;
+        const size_t hist = (size_t)e->subband.dev[dev].hist * d.bpc;
         const size_t keep_from = (d.consumed > hist ? d.consumed - hist : 0) & ~(size_t)15;
         const size_t rem = d.fill - keep_from;
         if (rem + nbytes > d.cap) {
@@ -1597,55 +1672,41 @@ int abg_fft_path(const abg_engine* e, int dev) {
 
 // ---- band spectrum monitor (definition in airband_b200.h) -------------------------------------------------------------
 int abg_spectrum_configure(abg_engine* e, int dev, int frame_stride) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_spectrum_configure: device %d out of range", dev);
+    SpecDev* d = monitor_dev(e, e->spectrum, dev, __func__);
+    if (!d) return ABG_ERANGE;
     if (frame_stride < 0) return fail(ABG_EINVAL, "abg_spectrum_configure: frame_stride %d is negative", frame_stride);
-    Device& d = e->dev[dev];
-    if (frame_stride == d.spec_stride) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream));  // an enqueued spectrum kernel may still use the work buffer and the tables
+    if (frame_stride == d->stride) return ABG_OK;
+    int rc = monitor_configure(e, e->spectrum, frame_stride > 0);  // an enqueued spectrum kernel may still use the work buffer
+    if (rc != ABG_OK) return rc;
     const int N = e->N, B = e->B, nbmax = e->nbmax;
-    if (d.spec_work) cudaFree(d.spec_work);
-    d.spec_work = nullptr;
-    d.spec_stride = d.spec_n_sel = d.spec_chunks = 0;
+    d->work.free();
+    d->stride = d->n_sel = d->chunks = 0;
     if (frame_stride > 0) {
-        if (monitor_on(e, e->spectrum) != ABG_OK) return ABG_ECUDA;
-        if (!d.spec_q.alloc(nbmax + 2, sizeof(float) * N)) return fail(ABG_ENOMEM, "Out of page-locked host memory for the spectrum ring");
+        if (!d->q.reserve(nbmax, sizeof(float) * N)) return fail(ABG_ENOMEM, "Out of page-locked host memory for the spectrum ring");
         const int n_sel = (B + frame_stride - 1) / frame_stride;
         const int chunks = (n_sel + ABG_SPEC_FPC - 1) / ABG_SPEC_FPC;
         const size_t sums = sizeof(float) * (size_t)nbmax * chunks * N;
-        if (cudaMalloc(&d.spec_work, sums + sizeof(int32_t) * nbmax) != cudaSuccess) {
-            d.spec_work = nullptr;
-            return fail(ABG_ENOMEM, "Out of device memory for the spectrum of device %d", dev);
-        }
-        CU(cudaMemset(static_cast<char*>(d.spec_work) + sums, 0, sizeof(int32_t) * nbmax));
-        d.spec_stride = frame_stride;
-        d.spec_n_sel = n_sel;
-        d.spec_chunks = chunks;
+        if (d->work.alloc(sums + sizeof(int32_t) * nbmax)) return fail(ABG_ENOMEM, "Out of device memory for the spectrum of device %d", dev);
+        CU(cudaMemset(d->work.p + sums, 0, sizeof(int32_t) * nbmax));
+        d->stride = frame_stride;
+        d->n_sel = n_sel;
+        d->chunks = chunks;
     }
-    // rebuild the launch's device list and its static table
-    std::vector<int> devs;
-    std::vector<SpecCfg> cfgs;
-    for (int i = 0; i < (int)e->dev.size(); i++) {
-        const Device& x = e->dev[i];
-        if (x.spec_stride <= 0) continue;
-        SpecCfg c{};
+    return monitor_publish(e, e->spectrum, [&](const Device& x, const SpecDev& s, SpecCfg& c) -> int {
         c.wsc = e->groups[x.group].wsc.p;
-        c.partial = static_cast<float*>(x.spec_work);
-        c.counter = reinterpret_cast<int32_t*>(static_cast<char*>(x.spec_work) + sizeof(float) * (size_t)nbmax * x.spec_chunks * N);
-        CU(cudaHostGetDevicePointer((void**)&c.ring, x.spec_q.ring, 0));
-        c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = x.spec_stride; c.n_sel = x.spec_n_sel; c.n_chunks = x.spec_chunks;
-        c.ring_cap = nbmax + 2;
-        devs.push_back(i);
-        cfgs.push_back(c);
-    }
-    return monitor_publish(e, e->spectrum, devs, cfgs);
+        c.partial = reinterpret_cast<float*>(s.work.p);
+        c.counter = reinterpret_cast<int32_t*>(s.work.p + sizeof(float) * (size_t)nbmax * s.chunks * N);
+        CU(cudaHostGetDevicePointer((void**)&c.ring, s.q.ring, 0));
+        c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = s.stride; c.n_sel = s.n_sel; c.n_chunks = s.chunks;
+        c.ring_cap = s.q.cap;
+        return ABG_OK;
+    });
 }
 
 int abg_fetch_spectrum(abg_engine* e, int dev, float* power, uint64_t* batch_seq, int32_t* n_frames) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_spectrum: device %d out of range", dev);
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int rc = monitor_pop(e, e->dev[dev].spec_q, e->spectrum, &src, &r);
+    const int rc = monitor_fetch(e, e->spectrum, dev, 0, __func__, &src, &r);
     if (rc <= 0) return rc;
     if (power) memcpy(power, src, sizeof(float) * e->N);
     if (batch_seq) *batch_seq = r.seq;
@@ -1657,39 +1718,28 @@ int abg_debug_spectrum_time(abg_engine* e, float* ms) { return monitor_time(e, e
 
 // ---- carrier frequency meter (definition in airband_b200.h) -----------------------------------------------------------
 int abg_carrier_configure(abg_engine* e, int dev, int on) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_carrier_configure: device %d out of range", dev);
+    CarDev* d = monitor_dev(e, e->carrier, dev, __func__);
+    if (!d) return ABG_ERANGE;
     if (on != 0 && on != 1) return fail(ABG_EINVAL, "abg_carrier_configure: on = %d is neither 0 nor 1", on);
-    Device& d = e->dev[dev];
-    if ((on == 1) == d.car_on) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream));  // an enqueued meter kernel may still read the device table
-    if (on) {
-        if (monitor_on(e, e->carrier) != ABG_OK) return ABG_ECUDA;
-        if (!d.car_q.alloc(e->nbmax + 2, sizeof(float) * 3 * (size_t)std::max(d.C, 1))) return fail(ABG_ENOMEM, "Out of page-locked host memory for the carrier meter ring");
-    }
-    d.car_on = on == 1;
-    // rebuild the launch's device list and its static table
-    std::vector<int> devs;
-    std::vector<CarCfg> cfgs;
-    for (int i = 0; i < (int)e->dev.size(); i++) {
-        const Device& x = e->dev[i];
-        if (!x.car_on) continue;
-        CarCfg c{};
-        CU(cudaHostGetDevicePointer((void**)&c.ring, x.car_q.ring, 0));
-        c.g0 = x.g0; c.n_channels = x.C; c.ring_cap = x.car_q.cap;
-        devs.push_back(i);
-        cfgs.push_back(c);
-    }
-    return monitor_publish(e, e->carrier, devs, cfgs);
+    if ((on == 1) == d->enabled) return ABG_OK;
+    const int rc = monitor_configure(e, e->carrier, on == 1);
+    if (rc != ABG_OK) return rc;
+    if (on && !d->q.reserve(e->nbmax, sizeof(float) * 3 * (size_t)std::max(e->dev[dev].C, 1)))
+        return fail(ABG_ENOMEM, "Out of page-locked host memory for the carrier meter ring");
+    d->enabled = on == 1;
+    return monitor_publish(e, e->carrier, [](const Device& x, const CarDev& s, CarCfg& c) -> int {
+        CU(cudaHostGetDevicePointer((void**)&c.ring, s.q.ring, 0));
+        c.g0 = x.g0; c.n_channels = x.C; c.ring_cap = s.q.cap;
+        return ABG_OK;
+    });
 }
 
 int abg_fetch_carrier(abg_engine* e, int dev, float* lag1, float* energy, uint64_t* batch_seq) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_carrier: device %d out of range", dev);
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int C = e->dev[dev].C;
-    const int rc = monitor_pop(e, e->dev[dev].car_q, e->carrier, &src, &r);
+    const int rc = monitor_fetch(e, e->carrier, dev, 0, __func__, &src, &r);
     if (rc <= 0) return rc;
+    const int C = e->dev[dev].C;
     if (lag1) memcpy(lag1, src, sizeof(float) * 2 * C);
     if (energy) memcpy(energy, src + sizeof(float) * 2 * C, sizeof(float) * C);
     if (batch_seq) *batch_seq = r.seq;
@@ -1700,55 +1750,42 @@ int abg_debug_carrier_time(abg_engine* e, float* ms) { return monitor_time(e, e-
 
 // ---- input level meter (definition in airband_b200.h) -----------------------------------------------------------------
 int abg_input_meter_configure(abg_engine* e, int dev, int on) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_input_meter_configure: device %d out of range", dev);
+    InmDev* d = monitor_dev(e, e->input_meter, dev, __func__);
+    if (!d) return ABG_ERANGE;
     if (on != 0 && on != 1) return fail(ABG_EINVAL, "abg_input_meter_configure: on = %d is neither 0 nor 1", on);
-    Device& d = e->dev[dev];
-    if ((on == 1) == d.inm_on) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream));  // an enqueued meter kernel may still read the device table
+    if ((on == 1) == d->enabled) return ABG_OK;
+    int rc = monitor_configure(e, e->input_meter, on == 1);
+    if (rc != ABG_OK) return rc;
     const int nbmax = e->nbmax;
-    const int chunks = abg_input_meter_chunks(e->B * d.hop_bytes);
     const size_t hist_bytes = sizeof(uint32_t) * 512 * (size_t)nbmax, counter_bytes = sizeof(int32_t) * (size_t)nbmax;
     const size_t part_off = (hist_bytes + counter_bytes + 15) & ~(size_t)15;
     if (on) {
-        if (monitor_on(e, e->input_meter) != ABG_OK) return ABG_ECUDA;
-        if (!d.inm_q.alloc(nbmax + 2, sizeof(abg_input_levels))) return fail(ABG_ENOMEM, "Out of page-locked host memory for the input meter ring");
-        if (!d.inm_work) {
+        if (!d->q.reserve(nbmax, sizeof(abg_input_levels))) return fail(ABG_ENOMEM, "Out of page-locked host memory for the input meter ring");
+        const int chunks = abg_input_meter_chunks(e->B * e->dev[dev].hop_bytes);
+        if (!d->work.p) {
             // histograms and counters start at zero; every launch leaves them at zero again
-            if (cudaMalloc(&d.inm_work, part_off + sizeof(long long) * ABG_INM_PARTIAL * (size_t)nbmax * chunks) != cudaSuccess) {
-                d.inm_work = nullptr;
+            if (d->work.alloc(part_off + sizeof(long long) * ABG_INM_PARTIAL * (size_t)nbmax * chunks))
                 return fail(ABG_ENOMEM, "Out of device memory for the input meter of device %d", dev);
-            }
-            CU(cudaMemset(d.inm_work, 0, part_off));
+            CU(cudaMemset(d->work.p, 0, part_off));
         }
-        d.inm_chunks = chunks;
+        d->chunks = chunks;
     }
-    d.inm_on = on == 1;
-    // rebuild the launch's device list and its static table
-    std::vector<int> devs;
-    std::vector<InmCfg> cfgs;
-    for (int i = 0; i < (int)e->dev.size(); i++) {
-        const Device& x = e->dev[i];
-        if (!x.inm_on) continue;
-        InmCfg c{};
-        CU(cudaHostGetDevicePointer((void**)&c.ring, x.inm_q.ring, 0));
-        char* w = static_cast<char*>(x.inm_work);
-        c.hist = reinterpret_cast<uint32_t*>(w);
-        c.counter = reinterpret_cast<int32_t*>(w + hist_bytes);
-        c.partial = reinterpret_cast<long long*>(w + part_off);
-        c.sfmt = x.sfmt; c.hop_bytes = x.hop_bytes; c.n_chunks = x.inm_chunks; c.ring_cap = x.inm_q.cap;
+    d->enabled = on == 1;
+    return monitor_publish(e, e->input_meter, [&](const Device& x, const InmDev& s, InmCfg& c) -> int {
+        CU(cudaHostGetDevicePointer((void**)&c.ring, s.q.ring, 0));
+        c.hist = reinterpret_cast<uint32_t*>(s.work.p);
+        c.counter = reinterpret_cast<int32_t*>(s.work.p + hist_bytes);
+        c.partial = reinterpret_cast<long long*>(s.work.p + part_off);
+        c.sfmt = x.sfmt; c.hop_bytes = x.hop_bytes; c.n_chunks = s.chunks; c.ring_cap = s.q.cap;
         c.scale = 1.0f / x.fullscale;
-        devs.push_back(i);
-        cfgs.push_back(c);
-    }
-    return monitor_publish(e, e->input_meter, devs, cfgs);
+        return ABG_OK;
+    });
 }
 
 int abg_fetch_input_levels(abg_engine* e, int dev, abg_input_levels* out) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_input_levels: device %d out of range", dev);
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int rc = monitor_pop(e, e->dev[dev].inm_q, e->input_meter, &src, &r);
+    const int rc = monitor_fetch(e, e->input_meter, dev, 0, __func__, &src, &r);
     if (rc <= 0) return rc;
     if (out) {
         memcpy(out, src, sizeof(abg_input_levels));
@@ -1786,35 +1823,29 @@ static uint32_t subband_coefficients(double offset_hz, int sample_rate, int n_co
 }
 
 int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int decim, int n_coeffs, const float* coeffs) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_subband_configure: device %d out of range", dev);
+    SbDev* s = monitor_dev(e, e->subband, dev, __func__);
+    if (!s) return ABG_ERANGE;
     if (k < 0 || k >= ABG_SUBBAND_MAX) return fail(ABG_ERANGE, "abg_subband_configure: output %d out of range [0, %d)", k, ABG_SUBBAND_MAX);
-    Device& d = e->dev[dev];
+    const Device& d = e->dev[dev];
     const int n = e->B * d.hop;  // samples per batch
     if (decim < 0 || decim > n) return fail(ABG_EINVAL, "abg_subband_configure: decimation %d outside [0, %d]", decim, n);
     if (decim > 0) {
         const int rc = subband_check("abg_subband_configure", d, n, offset_hz, decim, n_coeffs, coeffs);
         if (rc != ABG_OK) return rc;
     }
-    Device::Subband& so = d.sb[k];
+    SbDev::Output& so = s->out[k];
     if (decim == 0 && !so.on) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream));  // an enqueued kernel may still read the tables, the coefficients or the ring
+    const int rc = monitor_configure(e, e->subband, decim > 0);  // an enqueued kernel may still read the coefficients or the ring
+    if (rc != ABG_OK) return rc;
     if (decim > 0) {
-        if (monitor_on(e, e->subband) != ABG_OK) return ABG_ECUDA;
         std::vector<float2> g;
         const uint32_t delta = subband_coefficients(offset_hz, d.sample_rate, n_coeffs, coeffs, g);
-        if (so.coef_cap < n_coeffs) {
-            if (so.coef) cudaFree(so.coef);
-            so.coef = nullptr;
-            so.coef_cap = 0;
-            if (cudaMalloc((void**)&so.coef, sizeof(float2) * n_coeffs) != cudaSuccess) {
-                so.coef = nullptr;
-                return fail(ABG_ENOMEM, "Out of device memory for the sub-band coefficients of device %d", dev);
-            }
-            so.coef_cap = n_coeffs;
+        if (so.coef.n < (size_t)n_coeffs) {
+            so.coef.free();
+            if (so.coef.alloc(n_coeffs)) return fail(ABG_ENOMEM, "Out of device memory for the sub-band coefficients of device %d", dev);
         }
-        CU(cudaMemcpy(so.coef, g.data(), sizeof(float2) * n_coeffs, cudaMemcpyHostToDevice));
-        if (!so.q.reserve(e->nbmax + 2, sizeof(float2) * (size_t)((n + decim - 1) / decim)))
+        CU(cudaMemcpy(so.coef.p, g.data(), sizeof(float2) * n_coeffs, cudaMemcpyHostToDevice));
+        if (!so.q.reserve(e->nbmax, sizeof(float2) * (size_t)((n + decim - 1) / decim)))
             return fail(ABG_ENOMEM, "Out of page-locked host memory for the sub-band ring");
         so.decim = decim;
         so.n_coeffs = n_coeffs;
@@ -1822,43 +1853,34 @@ int abg_subband_configure(abg_engine* e, int dev, int k, double offset_hz, int d
         so.restart = true;
     }
     so.on = decim > 0;
-    d.sb_hist = 0;
-    for (const auto& x : d.sb)
-        if (x.on) d.sb_hist = std::max(d.sb_hist, x.n_coeffs - 1);
-    // rebuild the launch's device list and its static table
-    std::vector<int> devs;
-    e->sb_max_hist = 0;
-    std::vector<SbCfg> cfgs;
-    for (int i = 0; i < (int)e->dev.size(); i++) {
-        const Device& x = e->dev[i];
-        SbCfg c{};
-        for (const auto& y : x.sb) {
-            if (!y.on) continue;
-            SbOut& o = c.out[c.n_out++];
-            o.coef = y.coef;
-            CU(cudaHostGetDevicePointer((void**)&o.ring, y.q.ring, 0));
-            o.delta = y.delta; o.decim = y.decim; o.n_coeffs = y.n_coeffs;
-            o.ring_cap = y.q.cap; o.entry_bytes = (int32_t)y.q.entry_bytes;
+    s->hist = 0;
+    for (const auto& x : s->out)
+        if (x.on) s->hist = std::max(s->hist, x.n_coeffs - 1);
+    e->subband.max_hist = 0;
+    return monitor_publish(e, e->subband, [&](const Device& x, const SbDev& y, SbCfg& c) -> int {
+        for (const auto& o : y.out) {
+            if (!o.on) continue;
+            SbOut& w = c.out[c.n_out++];
+            w.coef = o.coef.p;
+            CU(cudaHostGetDevicePointer((void**)&w.ring, o.q.ring, 0));
+            w.delta = o.delta; w.decim = o.decim; w.n_coeffs = o.n_coeffs;
+            w.ring_cap = o.q.cap; w.entry_bytes = (int32_t)o.q.entry_bytes;
         }
-        if (c.n_out == 0) continue;
         c.sfmt = x.sfmt; c.bpc = x.bpc; c.batch_samples = e->B * x.hop; c.n_chunks = abg_subband_chunks(c.batch_samples);
-        c.hist = x.sb_hist;
+        c.hist = y.hist;
         c.scale = 1.0f / x.fullscale;
-        e->sb_max_hist = std::max(e->sb_max_hist, x.sb_hist);
-        devs.push_back(i);
-        cfgs.push_back(c);
-    }
-    return monitor_publish(e, e->subband, devs, cfgs);
+        e->subband.max_hist = std::max(e->subband.max_hist, y.hist);
+        return ABG_OK;
+    });
 }
 
 int abg_fetch_subband(abg_engine* e, int dev, int k, float* iq, uint64_t* batch_seq, uint64_t* first_index, int32_t* n_samples) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_subband: device %d out of range", dev);
     if (k < 0 || k >= ABG_SUBBAND_MAX) return fail(ABG_ERANGE, "abg_fetch_subband: output %d out of range [0, %d)", k, ABG_SUBBAND_MAX);
-    const Device& d = e->dev[dev];
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int rc = monitor_pop(e, e->dev[dev].sb[k].q, e->subband, &src, &r);
+    const int rc = monitor_fetch(e, e->subband, dev, k, __func__, &src, &r);
     if (rc <= 0) return rc;
+    const Device& d = e->dev[dev];
     // the batch's outputs: s0 <= mD < s0 + n with D the decimation the batch was computed with
     const unsigned long long n = (unsigned long long)e->B * d.hop, D = (unsigned long long)r.aux;
     const unsigned long long s0 = ((unsigned long long)ABG_AGC_EXTRA + r.seq * e->B) * d.hop;
@@ -1874,75 +1896,61 @@ int abg_debug_subband_time(abg_engine* e, float* ms) { return monitor_time(e, e-
 
 // ---- CTCSS tone meter (definition in airband_b200.h) -------------------------------------------------------------------
 // The tone table of the current list: T[j][2k] = cos, T[j][2k+1] = -sin of 2 pi (delta_k j mod 2^32) / 2^32, built in double
-// and rounded once to float32; columns 2K .. tm_cols are zero.  The caller has waited for stream B.
+// and rounded once to float32; columns 2K .. cols are zero.  The caller has waited for stream B.
 static int tone_meter_table(abg_engine* e) {
-    const int K = (int)e->tm_freqs.size(), B = e->B;
+    ToneMeterLaunch& m = e->tone_meter;
+    const int K = (int)m.freqs.size(), B = e->B;
     const int cols = (2 * K + ABG_TM_COLS - 1) / ABG_TM_COLS * ABG_TM_COLS;
-    e->tm_delta.resize(K);
+    m.delta.resize(K);
     for (int k = 0; k < K; k++)
-        e->tm_delta[k] = (uint32_t)(unsigned long long)llround((double)e->tm_freqs[k] / e->W * 4294967296.0);
+        m.delta[k] = (uint32_t)(unsigned long long)llround((double)m.freqs[k] / e->W * 4294967296.0);
     std::vector<float> t((size_t)B * cols, 0.0f);
     for (int j = 0; j < B; j++)
         for (int k = 0; k < K; k++) {
-            const double turns = (double)(int32_t)(e->tm_delta[k] * (uint32_t)j) * 0x1p-32;  // exact, in [-1/2, 1/2)
+            const double turns = (double)(int32_t)(m.delta[k] * (uint32_t)j) * 0x1p-32;  // exact, in [-1/2, 1/2)
             t[(size_t)j * cols + 2 * k] = (float)cos(2.0 * M_PI * turns);
             t[(size_t)j * cols + 2 * k + 1] = (float)-sin(2.0 * M_PI * turns);
         }
-    if (cols != e->tm_cols) {
-        e->tm_table.free();
-        e->tm_cols = 0;
-        if (e->tm_table.alloc(t.size())) {
-            e->tm_table.p = nullptr;
-            return fail(ABG_ENOMEM, "Out of device memory for the tone meter table");
-        }
-        e->tm_cols = cols;
+    if (cols != m.cols) {
+        m.table.free();
+        m.cols = 0;
+        if (m.table.alloc(t.size())) return fail(ABG_ENOMEM, "Out of device memory for the tone meter table");
+        m.cols = cols;
     }
-    CU(cudaMemcpy(e->tm_table.p, t.data(), sizeof(float) * t.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(m.table.p, t.data(), sizeof(float) * t.size(), cudaMemcpyHostToDevice));
     return ABG_OK;
 }
 
 int abg_tone_meter_configure(abg_engine* e, int dev, int on) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_tone_meter_configure: device %d out of range", dev);
+    ToneMeterLaunch& m = e->tone_meter;
+    TmDev* d = monitor_dev(e, m, dev, __func__);
+    if (!d) return ABG_ERANGE;
     if (on != 0 && on != 1) return fail(ABG_EINVAL, "abg_tone_meter_configure: on = %d is neither 0 nor 1", on);
-    Device& d = e->dev[dev];
-    if ((on == 1) == d.tm_on) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream_b));  // an enqueued meter kernel may still read the device tables
+    if ((on == 1) == d->enabled) return ABG_OK;
+    int rc = monitor_configure(e, m, on == 1);
+    if (rc != ABG_OK) return rc;
     if (on) {
-        if (monitor_on(e, e->tone_meter) != ABG_OK) return ABG_ECUDA;
-        if (!d.tm_q.alloc(e->nbmax + 2, sizeof(float) * (2 * ABG_TONE_MAX + 2) * (size_t)std::max(d.C, 1)))
+        if (!d->q.reserve(e->nbmax, sizeof(float) * (2 * ABG_TONE_MAX + 2) * (size_t)std::max(e->dev[dev].C, 1)))
             return fail(ABG_ENOMEM, "Out of page-locked host memory for the tone meter ring");
-        if (!e->tm_table.p) {
-            const int rc = tone_meter_table(e);
-            if (rc != ABG_OK) return rc;
-        }
+        if (!m.table.p && (rc = tone_meter_table(e)) != ABG_OK) return rc;
     }
-    d.tm_on = on == 1;
-    // rebuild the launch's device list, its static table and the channel map
-    std::vector<int> devs;
-    std::vector<TmCfg> cfgs;
-    std::vector<int32_t> chan_dev;
-    for (int i = 0; i < (int)e->dev.size(); i++) {
-        const Device& x = e->dev[i];
-        if (!x.tm_on) continue;
-        TmCfg c{};
-        CU(cudaHostGetDevicePointer((void**)&c.ring, x.tm_q.ring, 0));
-        c.g0 = x.g0; c.n_channels = x.C; c.first = (int32_t)chan_dev.size(); c.ring_cap = x.tm_q.cap;
-        chan_dev.insert(chan_dev.end(), x.C, (int32_t)devs.size());
-        devs.push_back(i);
-        cfgs.push_back(c);
-    }
-    e->tm_chan_dev.free();
-    e->tm_n_chan = 0;
-    if (!chan_dev.empty()) {
-        if (e->tm_chan_dev.alloc(chan_dev.size())) {
-            e->tm_chan_dev.p = nullptr;
-            return fail(ABG_ENOMEM, "Out of device memory for the tone meter tables");
-        }
-        CU(cudaMemcpy(e->tm_chan_dev.p, chan_dev.data(), sizeof(int32_t) * chan_dev.size(), cudaMemcpyHostToDevice));
-        e->tm_n_chan = (int)chan_dev.size();
-    }
-    return monitor_publish(e, e->tone_meter, devs, cfgs);
+    d->enabled = on == 1;
+    std::vector<int32_t> chan_dev;  // the channel map
+    int32_t k = 0;
+    rc = monitor_publish(e, m, [&](const Device& x, const TmDev& s, TmCfg& c) -> int {
+        CU(cudaHostGetDevicePointer((void**)&c.ring, s.q.ring, 0));
+        c.g0 = x.g0; c.n_channels = x.C; c.first = (int32_t)chan_dev.size(); c.ring_cap = s.q.cap;
+        chan_dev.insert(chan_dev.end(), x.C, k++);
+        return ABG_OK;
+    });
+    if (rc != ABG_OK) return rc;
+    m.chan_dev.free();
+    m.n_chan = 0;
+    if (chan_dev.empty()) return ABG_OK;
+    if (m.chan_dev.alloc(chan_dev.size())) return fail(ABG_ENOMEM, "Out of device memory for the tone meter tables");
+    CU(cudaMemcpy(m.chan_dev.p, chan_dev.data(), sizeof(int32_t) * chan_dev.size(), cudaMemcpyHostToDevice));
+    m.n_chan = (int)chan_dev.size();
+    return ABG_OK;
 }
 
 int abg_tone_meter_set_tones(abg_engine* e, int n_tones, const float* freqs) {
@@ -1956,19 +1964,17 @@ int abg_tone_meter_set_tones(abg_engine* e, int n_tones, const float* freqs) {
                 return fail(ABG_EINVAL, "abg_tone_meter_set_tones: tone %d (%g Hz) outside (0, %d) Hz", k, (double)freqs[k], e->W / 2);
     }
     cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream_b));  // an enqueued meter kernel may still read the table
-    e->tm_freqs = list;
-    return e->tm_table.p ? tone_meter_table(e) : ABG_OK;
+    CU(cudaStreamSynchronize(monitor_stream(e, e->tone_meter)));  // an enqueued meter kernel may still read the table
+    e->tone_meter.freqs = list;
+    return e->tone_meter.table.p ? tone_meter_table(e) : ABG_OK;
 }
 
 int abg_fetch_tone_meter(abg_engine* e, int dev, float* tones, float* energy, int32_t* active, uint64_t* batch_seq, int32_t* n_tones) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_tone_meter: device %d out of range", dev);
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const size_t C = (size_t)e->dev[dev].C;
-    const int rc = monitor_pop(e, e->dev[dev].tm_q, e->tone_meter, &src, &r);
+    const int rc = monitor_fetch(e, e->tone_meter, dev, 0, __func__, &src, &r);
     if (rc <= 0) return rc;
-    const size_t K = (size_t)r.aux;
+    const size_t C = (size_t)e->dev[dev].C, K = (size_t)r.aux;
     if (tones) memcpy(tones, src, sizeof(float) * 2 * K * C);
     if (energy) memcpy(energy, src + sizeof(float) * 2 * K * C, sizeof(float) * C);
     if (active) memcpy(active, src + sizeof(float) * (2 * K + 1) * C, sizeof(int32_t) * C);
@@ -1981,10 +1987,11 @@ int abg_debug_tone_meter_time(abg_engine* e, float* ms) { return monitor_time(e,
 
 // ---- band activity detector (definition in airband_b200.h) ----------------------------------------------------------
 int abg_activity_configure(abg_engine* e, int dev, int stride, int hang, int min_span, const float* thr) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_activity_configure: device %d out of range", dev);
+    ActDev* d = monitor_dev(e, e->activity, dev, __func__);
+    if (!d) return ABG_ERANGE;
     if (stride < 0 || hang < 0 || min_span < 0)
         return fail(ABG_EINVAL, "abg_activity_configure: negative argument (stride %d, hang %d, min_span %d)", stride, hang, min_span);
-    const int N = e->N, B = e->B, nbmax = e->nbmax;
+    const int N = e->N, B = e->B;
     if (stride > 0) {
         if (stride > B) return fail(ABG_EINVAL, "abg_activity_configure: stride %d exceeds the batch of %d frames", stride, B);
         const int n_sel = (B + stride - 1) / stride;
@@ -1995,52 +2002,38 @@ int abg_activity_configure(abg_engine* e, int dev, int stride, int hang, int min
             if (!std::isfinite(thr[k]) || !(thr[k] > 0.0f))
                 return fail(ABG_EINVAL, "abg_activity_configure: threshold of bin %d (%g) is not finite and positive", k, (double)thr[k]);
     }
-    Device& d = e->dev[dev];
-    if (stride == 0 && d.act_stride == 0) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream));  // an enqueued detector kernel may still read the thresholds and the tables
+    if (stride == 0 && d->stride == 0) return ABG_OK;
+    const int rc = monitor_configure(e, e->activity, stride > 0);  // an enqueued detector kernel may still read the thresholds
+    if (rc != ABG_OK) return rc;
     if (stride > 0) {
-        if (monitor_on(e, e->activity) != ABG_OK) return ABG_ECUDA;
-        if (!d.act_q.alloc(nbmax + 2, ABG_ACT_HEAD_BYTES + sizeof(abg_burst) * (size_t)ABG_ACTIVITY_MAX_RECORDS))
+        if (!d->q.reserve(e->nbmax, ABG_ACT_HEAD_BYTES + sizeof(abg_burst) * (size_t)ABG_ACTIVITY_MAX_RECORDS))
             return fail(ABG_ENOMEM, "Out of page-locked host memory for the activity ring");
-        if (!d.act_thr && cudaMalloc((void**)&d.act_thr, sizeof(float) * N) != cudaSuccess) {
-            d.act_thr = nullptr;
-            return fail(ABG_ENOMEM, "Out of device memory for the activity thresholds of device %d", dev);
-        }
-        CU(cudaMemcpy(d.act_thr, thr, sizeof(float) * N, cudaMemcpyHostToDevice));
-        d.act_n_sel = (B + stride - 1) / stride;
+        if (!d->thr.p && d->thr.alloc(N)) return fail(ABG_ENOMEM, "Out of device memory for the activity thresholds of device %d", dev);
+        CU(cudaMemcpy(d->thr.p, thr, sizeof(float) * N, cudaMemcpyHostToDevice));
+        d->n_sel = (B + stride - 1) / stride;
     }
-    d.act_stride = stride;
-    d.act_hang = stride > 0 ? hang : 0;
-    d.act_min_span = stride > 0 ? min_span : 0;
-    // rebuild the launch's device list and its static table
-    std::vector<int> devs;
-    std::vector<ActCfg> cfgs;
-    for (int i = 0; i < (int)e->dev.size(); i++) {
-        const Device& x = e->dev[i];
-        if (x.act_stride <= 0) continue;
-        ActCfg c{};
+    d->stride = stride;
+    d->hang = stride > 0 ? hang : 0;
+    d->min_span = stride > 0 ? min_span : 0;
+    return monitor_publish(e, e->activity, [&](const Device& x, const ActDev& s, ActCfg& c) -> int {
         c.wsc = e->groups[x.group].wsc.p;
-        c.thr = x.act_thr;
-        CU(cudaHostGetDevicePointer((void**)&c.ring, x.act_q.ring, 0));
-        c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = x.act_stride; c.n_sel = x.act_n_sel;
-        c.hang = x.act_hang; c.min_span = x.act_min_span;
-        c.ring_cap = x.act_q.cap; c.entry_bytes = (int32_t)x.act_q.entry_bytes;
-        devs.push_back(i);
-        cfgs.push_back(c);
-    }
-    return monitor_publish(e, e->activity, devs, cfgs);
+        c.thr = s.thr.p;
+        CU(cudaHostGetDevicePointer((void**)&c.ring, s.q.ring, 0));
+        c.hop_bytes = x.hop_bytes; c.sfmt = x.sfmt; c.stride = s.stride; c.n_sel = s.n_sel;
+        c.hang = s.hang; c.min_span = s.min_span;
+        c.ring_cap = s.q.cap; c.entry_bytes = (int32_t)s.q.entry_bytes;
+        return ABG_OK;
+    });
 }
 
 static_assert(sizeof(abg_burst) == 40, "abg_burst has a fixed 40-byte layout");
 
 int abg_fetch_activity(abg_engine* e, int dev, abg_burst* out, int cap, int32_t* n_stored, int32_t* n_total, uint64_t* batch_seq,
                        int32_t* settings3) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_fetch_activity: device %d out of range", dev);
     if (cap < 0) return fail(ABG_EINVAL, "abg_fetch_activity: cap %d is negative", cap);
     const unsigned char* src = nullptr;
     MonitorQueue::Entry r{};
-    const int rc = monitor_pop(e, e->dev[dev].act_q, e->activity, &src, &r);
+    const int rc = monitor_fetch(e, e->activity, dev, 0, __func__, &src, &r);
     if (rc <= 0) return rc;
     int32_t head[4];
     memcpy(head, src, sizeof(head));
@@ -2066,125 +2059,114 @@ int abg_debug_activity_time(abg_engine* e, float* ms) { return monitor_time(e, e
 constexpr long long kHistoryCaptureChunk = 1 << 20;  // outputs per capture launch: the output scratch is 8 MB
 
 int abg_history_configure(abg_engine* e, int dev, int n_batches) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_configure: device %d out of range", dev);
+    HiDev* h = monitor_dev(e, e->history, dev, __func__);
+    if (!h) return ABG_ERANGE;
     if (n_batches < 0) return fail(ABG_EINVAL, "abg_history_configure: n_batches %d is negative", n_batches);
-    Device& d = e->dev[dev];
-    if (n_batches == d.hi_batches) return ABG_OK;
-    cudaSetDevice(e->cuda_dev);
-    CU(cudaStreamSynchronize(e->stream));  // an enqueued append or capture may still use the ring and the tables
-    if (d.hi_ring) cudaFree(d.hi_ring);
-    d.hi_ring = nullptr;
-    d.hi_batches = 0;
-    d.hi_ring_bytes = d.hi_cap = d.hi_first = d.hi_end = 0;
-    int rc = ABG_OK;
+    if (n_batches == h->batches) return ABG_OK;
+    int rc = monitor_configure(e, e->history, n_batches > 0);  // an enqueued append or capture may still use the ring
+    if (rc != ABG_OK) return rc;
+    const Device& d = e->dev[dev];
+    h->ring.free();
+    h->batches = 0;
+    h->cap = h->first = h->end = 0;
     if (n_batches > 0) {
-        if (monitor_on(e, e->history) != ABG_OK) return ABG_ECUDA;
         const unsigned long long cap = (unsigned long long)n_batches * e->B * d.hop;
         const unsigned long long R = (cap * d.bpc + 15) & ~15ull;
-        if (cudaMalloc((void**)&d.hi_ring, R) != cudaSuccess) {
-            cudaGetLastError();  // not sticky: keep it from failing the next launch check
-            d.hi_ring = nullptr;
+        if (h->ring.alloc(R)) {
             rc = fail(ABG_ENOMEM, "Out of device memory for the I/Q history of device %d (%llu bytes)", dev, R);
         } else {
-            d.hi_batches = n_batches;
-            d.hi_cap = cap;
-            d.hi_ring_bytes = R;
+            h->batches = n_batches;
+            h->cap = cap;
         }
     }
-    // rebuild the launch's device list and its static table
-    std::vector<int> devs;
-    std::vector<HiCfg> cfgs;
-    for (int i = 0; i < (int)e->dev.size(); i++) {
-        const Device& x = e->dev[i];
-        if (!x.hi_ring) continue;
-        HiCfg c{};
-        c.ring = x.hi_ring;
-        c.ring_bytes = x.hi_ring_bytes;
-        devs.push_back(i);
-        cfgs.push_back(c);
-    }
-    const int rp = monitor_publish(e, e->history, devs, cfgs);
+    const int rp = monitor_publish(e, e->history, [](const Device&, const HiDev& s, HiCfg& c) -> int {
+        c.ring = s.ring.p;
+        c.ring_bytes = s.ring.n;
+        return ABG_OK;
+    });
     return rc != ABG_OK ? rc : rp;
 }
 
 int abg_history_range(abg_engine* e, int dev, uint64_t* first, uint64_t* end) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_range: device %d out of range", dev);
+    const HiDev* h = monitor_dev(e, e->history, dev, __func__);
+    if (!h) return ABG_ERANGE;
     if (!first || !end) return fail(ABG_EINVAL, "abg_history_range: null argument");
-    *first = e->dev[dev].hi_first;
-    *end = e->dev[dev].hi_end;
+    *first = h->first;
+    *end = h->end;
     return ABG_OK;
 }
 
 // [first, first + n) inside the device's history (n >= 1)
-static bool history_holds(const Device& d, unsigned __int128 first, unsigned __int128 n) {
-    return d.hi_first < d.hi_end && first >= d.hi_first && first + n <= d.hi_end;
+static bool history_holds(const HiDev& h, unsigned __int128 first, unsigned __int128 n) {
+    return h.first < h.end && first >= h.first && first + n <= h.end;
 }
 
 int abg_history_raw(abg_engine* e, int dev, uint64_t first, int64_t n, void* out) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_raw: device %d out of range", dev);
+    const HiDev* h = monitor_dev(e, e->history, dev, __func__);
+    if (!h) return ABG_ERANGE;
     if (n < 0 || (n > 0 && !out)) return fail(ABG_EINVAL, "abg_history_raw: %lld samples into %p", (long long)n, out);
-    const Device& d = e->dev[dev];
     if (n == 0) return ABG_OK;
-    if (!history_holds(d, first, (unsigned long long)n))
+    if (!history_holds(*h, first, (unsigned long long)n))
         return fail(ABG_ERANGE, "abg_history_raw: samples [%llu, +%lld) outside the history [%llu, %llu)", (unsigned long long)first,
-                    (long long)n, (unsigned long long)d.hi_first, (unsigned long long)d.hi_end);
+                    (long long)n, (unsigned long long)h->first, (unsigned long long)h->end);
     cudaSetDevice(e->cuda_dev);
     // on the K1 stream, behind the appends that wrote them; n <= capacity, so at most one wrap
-    const unsigned long long R = d.hi_ring_bytes, b0 = (unsigned long long)first * d.bpc % R, len = (unsigned long long)n * d.bpc;
+    const int bpc = e->dev[dev].bpc;
+    const unsigned long long R = h->ring.n, b0 = (unsigned long long)first * bpc % R, len = (unsigned long long)n * bpc;
     const unsigned long long len0 = std::min(len, R - b0);
-    CU(cudaMemcpyAsync(out, d.hi_ring + b0, len0, cudaMemcpyDeviceToHost, e->stream));
-    if (len0 < len) CU(cudaMemcpyAsync(static_cast<char*>(out) + len0, d.hi_ring, len - len0, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaMemcpyAsync(out, h->ring.p + b0, len0, cudaMemcpyDeviceToHost, e->stream));
+    if (len0 < len) CU(cudaMemcpyAsync(static_cast<char*>(out) + len0, h->ring.p, len - len0, cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
     return ABG_OK;
 }
 
 int abg_history_subband(abg_engine* e, int dev, double offset_hz, int decim, int n_coeffs, const float* coeffs, uint64_t first_m,
                         int64_t n_out, float* iq) {
-    if (dev < 0 || dev >= (int)e->dev.size()) return fail(ABG_ERANGE, "abg_history_subband: device %d out of range", dev);
+    HistoryLaunch& m = e->history;
+    const HiDev* h = monitor_dev(e, m, dev, __func__);
+    if (!h) return ABG_ERANGE;
     const Device& d = e->dev[dev];
     int rc = subband_check("abg_history_subband", d, e->B * d.hop, offset_hz, decim, n_coeffs, coeffs);
     if (rc != ABG_OK) return rc;
     if (n_out < 1 || !iq) return fail(ABG_EINVAL, "abg_history_subband: %lld outputs into %p", (long long)n_out, (void*)iq);
     // every tap in the history: first_m D - (L - 1) >= first and (first_m + n_out - 1) D < end
     const unsigned __int128 D = (unsigned)decim, lo = (unsigned __int128)first_m * D, hi = ((unsigned __int128)first_m + n_out - 1) * D;
-    if (d.hi_first == d.hi_end || lo < (unsigned __int128)d.hi_first + (n_coeffs - 1) || hi >= d.hi_end)
+    if (h->first == h->end || lo < (unsigned __int128)h->first + (n_coeffs - 1) || hi >= h->end)
         return fail(ABG_ERANGE, "abg_history_subband: outputs [%llu, +%lld) at decimation %d with %d coefficients read samples outside the history [%llu, %llu)",
-                    (unsigned long long)first_m, (long long)n_out, decim, n_coeffs, (unsigned long long)d.hi_first, (unsigned long long)d.hi_end);
+                    (unsigned long long)first_m, (long long)n_out, decim, n_coeffs, (unsigned long long)h->first, (unsigned long long)h->end);
     std::vector<float2> g;
     const uint32_t delta = subband_coefficients(offset_hz, d.sample_rate, n_coeffs, coeffs, g);
     cudaSetDevice(e->cuda_dev);
-    if (!e->hi_out.p) {
-        if (e->hi_coef.alloc(ABG_SUBBAND_MAX_COEFFS) || e->hi_out.alloc(kHistoryCaptureChunk)) {
-            cudaGetLastError();
-            e->hi_coef.free();
-            e->hi_out.free();
+    if (!m.out.p) {
+        if (m.coef.alloc(ABG_SUBBAND_MAX_COEFFS) || m.out.alloc(kHistoryCaptureChunk)) {
+            m.coef.free();
             return fail(ABG_ENOMEM, "Out of device memory for the I/Q history capture");
         }
-        for (auto& ev : e->hi_ev) CU(cudaEventCreate(&ev));
+        for (auto& ev : m.ev) CU(cudaEventCreate(&ev));
     }
     // on the K1 stream: behind every append it reads, and ahead of every later one that would overwrite its samples
-    CU(cudaMemcpyAsync(e->hi_coef.p, g.data(), sizeof(float2) * n_coeffs, cudaMemcpyHostToDevice, e->stream));
+    CU(cudaMemcpyAsync(m.coef.p, g.data(), sizeof(float2) * n_coeffs, cudaMemcpyHostToDevice, e->stream));
     HiCapture c{};
-    c.ring = d.hi_ring; c.ring_bytes = d.hi_ring_bytes; c.coef = e->hi_coef.p; c.out = e->hi_out.p;
+    c.ring = h->ring.p; c.ring_bytes = h->ring.n; c.coef = m.coef.p; c.out = m.out.p;
     c.decim = decim; c.n_coeffs = n_coeffs; c.sfmt = d.sfmt; c.delta = delta; c.scale = 1.0f / d.fullscale;
     float total_ms = 0.0f;
     for (long long done = 0; done < n_out;) {
         const long long cnt = std::min<long long>(kHistoryCaptureChunk, n_out - done);
         c.m0 = (long long)(first_m + (uint64_t)done);
         c.n_out = (int32_t)cnt;
-        CU(cudaEventRecord(e->hi_ev[0], e->stream));
+        CU(cudaEventRecord(m.ev[0], e->stream));
         const cudaError_t er = abg_launch_history_capture(c, e->stream);
         if (er != cudaSuccess) return fail(ABG_ECUDA, "I/Q history capture launch failed: %s", cudaGetErrorString(er));
         e->launches++;
-        CU(cudaEventRecord(e->hi_ev[1], e->stream));
-        CU(cudaMemcpyAsync(iq + 2 * done, e->hi_out.p, sizeof(float2) * cnt, cudaMemcpyDeviceToHost, e->stream));
+        CU(cudaEventRecord(m.ev[1], e->stream));
+        CU(cudaMemcpyAsync(iq + 2 * done, m.out.p, sizeof(float2) * cnt, cudaMemcpyDeviceToHost, e->stream));
         CU(cudaStreamSynchronize(e->stream));
         float ms = 0.0f;
-        CU(cudaEventElapsedTime(&ms, e->hi_ev[0], e->hi_ev[1]));
+        CU(cudaEventElapsedTime(&ms, m.ev[0], m.ev[1]));
         total_ms += ms;
         done += cnt;
     }
-    e->hi_capture_ms = total_ms;
+    m.capture_ms = total_ms;
     return ABG_OK;
 }
 
@@ -2192,7 +2174,7 @@ int abg_debug_history_time(abg_engine* e, float* ms2) {
     if (!ms2) return fail(ABG_EINVAL, "abg_debug_history_time: null argument");
     const int rc = monitor_time(e, e->history, ms2, __func__);
     if (rc != ABG_OK) return rc;
-    ms2[1] = e->hi_capture_ms;
+    ms2[1] = e->history.capture_ms;
     return ABG_OK;
 }
 

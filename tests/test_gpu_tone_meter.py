@@ -1,12 +1,9 @@
 """The CTCSS tone meter on the GPU (-m gpu): every reading against float64 sums of the fetched audio with the exact integer
 phase, bitwise reproducibility across run grouping and push sizes, identification of every standard tone in injected
-audio and in a pushed NFM stream, the five batch monitors together, and the lossy queue and its errors."""
-import itertools
-
+audio and in a pushed NFM stream, and the lossy queue and its errors."""
 import numpy as np
 import pytest
 
-import test_gpu_monitors as four
 from airband_b200 import config as cm
 from airband_b200 import lib
 from airband_b200 import workloads as wl
@@ -199,92 +196,6 @@ def test_identifies_subaudible_tones_in_a_pushed_nfm_stream():
         if f in (67.0, 69.3):  # the neighbour 2.3 Hz away (1.15 bins of the 0.5 s window) reads at most half of it
             other = 69.3 if f == 67.0 else 67.0
             assert share[lib.STANDARD_TONES.index(other)] < 0.5 * got[1]
-
-
-# ------------------------------------------------------------------------------------------------ all five monitors
-MONITORS = four.MONITORS + ("tone_meter",)
-SUBSETS = [frozenset(s) for n in range(len(MONITORS) + 1) for s in itertools.combinations(MONITORS, n)]
-
-
-def fetch_all_monitors(e):
-    got = four.fetch_monitors(e)
-    got["tone_meter"] = []
-    while (x := e.fetch_tone_meter(0)) is not None:
-        got["tone_meter"].append((x[0].view(np.uint64).copy(), x[1].view(np.uint32).copy(), x[2].copy(), x[3]))
-    return got
-
-
-def times(e):
-    return {**four.kernel_times(e), "tone_meter": e.tone_meter_time()}
-
-
-def drive(cfg, raw, monitors):
-    """test_gpu_monitors.drive with the tone meter as a fifth monitor."""
-    e = lib.Engine(cfg, max_batches_per_run=2, input_capacity_batches=3)
-    four.switch_on(e, cfg, monitors)
-    if "tone_meter" in monitors:
-        e.tone_meter_configure(0, True)
-    res = dict(audio=[], runs=[], launches=[], readings={m: [] for m in MONITORS}, times=[])
-    step = 2 * (cfg.wave_batch * cfg.hop(0) // 3 + 1)
-    pos = 0
-    while pos < raw.size or e.batches_available(0):
-        if pos < raw.size:
-            e.push(0, raw[pos:pos + step])
-            pos += step
-        l0 = e.launch_count()
-        n = e.run(-1)
-        if n == 0:
-            assert e.launch_count() == l0
-            continue
-        e.sync()
-        res["runs"].append(n)
-        res["launches"].append(e.launch_count() - l0)
-        res["times"].append(times(e))
-        while (g := e.fetch(0)) is not None:
-            res["audio"].append((g[0].view(np.uint32).copy(), g[1].view(np.uint64).copy(), g[2].copy()))
-        for m, got in fetch_all_monitors(e).items():
-            res["readings"][m] += got
-    res["stats"] = [tuple(getattr(e.stats(0, c), f) for f in four.STAT_FIELDS) for c in range(len(cfg.devices[0].channels))]
-    e.resident_load(0, raw[:e.resident_bytes_needed(0)])
-    res["resident_launches"] = []
-    for _ in range(3):
-        l0 = e.launch_count()
-        assert e.run_resident(2) == 2
-        e.sync()
-        res["resident_launches"].append(e.launch_count() - l0)
-        res["resident_times"] = times(e)
-    res["resident_queued"] = {m: len(got) for m, got in fetch_all_monitors(e).items()}
-    res["resident_audio"] = e.fetch(0)
-    e.close()
-    return res
-
-
-@pytest.fixture(scope="module")
-def runs():
-    cfg, raws = CASES["am_u8"](n_batches=6)
-    return {s: drive(cfg, raws[0], s) for s in SUBSETS}
-
-
-@pytest.mark.parametrize("subset", SUBSETS, ids=lambda s: "+".join(m for m in MONITORS if m in s) or "none")
-def test_every_subset_of_five_monitors(runs, subset):
-    off, got = runs[frozenset()], runs[subset]
-    assert got["runs"] == off["runs"] and len(off["runs"]) > 2
-    assert got["launches"] == [n + 2 * len(subset) for n in off["launches"]]
-    assert got["resident_launches"] == [n + 2 * len(subset) for n in off["resident_launches"]]
-    for t in got["times"] + [got["resident_times"]]:
-        assert {m for m, ms in t.items() if ms > 0.0} == set(subset), t
-    for m in MONITORS:
-        assert bool(got["readings"][m]) == (m in subset), m
-        if m in subset:
-            alone = runs[frozenset([m])]["readings"][m]
-            assert len(got["readings"][m]) == len(alone)
-            for a, b in zip(got["readings"][m], alone):
-                assert all(np.array_equal(x, y) for x, y in zip(a, b)), m
-    assert all(n == 0 for n in got["resident_queued"].values()) and got["resident_audio"] is None
-    assert len(got["audio"]) == len(off["audio"]) == sum(off["runs"])
-    for a, b in zip(got["audio"], off["audio"]):
-        assert all(np.array_equal(x, y) for x, y in zip(a, b))
-    assert got["stats"] == off["stats"]
 
 
 # --------------------------------------------------------------------------------------------------- queue and errors
