@@ -512,6 +512,47 @@ ABG_API int abg_history_subband(abg_engine* e, int dev, double offset_hz, int de
  * events on the K1 stream. */
 ABG_API int abg_debug_history_time(abg_engine* e, float* ms2);
 
+/* History replay (not part of the reference surface: it demodulates any frequency of a device's I/Q history to audio, as a
+ * channel configured there in advance would have, so that every transmission the activity detector finds can be heard).
+ * Job j replays device dev from batch first_batch (numbered as for the band spectrum) for n_batches batches through the
+ * engine's own K1 and K2.  Its outputs are bitwise what this fresh engine produces:
+ *   config   abg_create with this engine's fft_size, wave_rate and fm_demod, one device with dev's sfmt, fullscale and
+ *            sample_rate, and channels[n_channels] of the job;
+ *   options  this engine's cuda_device and fft_mode, everything else default;
+ *   input    dev's stream from sample S = first_batch * WAVE_BATCH * hop on (what abg_history_raw(e, dev, S, ...) returns),
+ *            run until it has produced n_batches batches.
+ * Frame AGC_EXTRA + b*WAVE_BATCH + i of that engine is frame AGC_EXTRA + (first_batch + b)*WAVE_BATCH + i of dev, so
+ * replayed batch b is dev's batch first_batch + b, demodulated from a fresh channel state.  The results do not depend on
+ * how many jobs share a call or their order, on max_batches_per_run, or on the push pattern the history was filled with.
+ * Every sample that engine reads must lie in the history: [S, S + (AGC_EXTRA + n_batches*WAVE_BATCH)*hop + fft_size - hop)
+ * inside abg_history_range (its last frame reaches fft_size - hop samples into the batch after the last one).  Several
+ * jobs may replay the same device.  Scan mode does not apply to replayed channels.
+ * Computed on the GPU: the engine keeps a private replay engine on the same CUDA device with one device per job, so all
+ * of a call's jobs share each K1 and K2 launch.  A gather kernel on the K1 stream moves the window's bytes from the history
+ * ring into that engine's input buffers (behind every append it reads, ahead of every later one that would overwrite
+ * them), in chunks of max_batches_per_run batches.  Nothing is allocated before the first replay; the replay engine is
+ * kept for later calls, grows only when a call needs more devices of a shape than it holds, and is freed when the last
+ * history is switched off.  Live runs, outputs and monitors are unaffected.
+ * The call waits for its results. */
+typedef struct abg_replay_job {
+    int32_t dev;                      /* device whose history is replayed */
+    int32_t n_batches;                /* >= 1 */
+    uint64_t first_batch;             /* dev's batch number of the first replayed batch */
+    int32_t n_channels;               /* >= 1 */
+    const abg_channel_cfg* channels;  /* as abg_create takes them */
+    float* waveout;                   /* [n_batches][n_channels][WAVE_BATCH], caller memory */
+    float* iq_out;                    /* [n_batches][n_channels][2*WAVE_BATCH] or NULL */
+    char* axcindicate;                /* [n_batches][n_channels] */
+    abg_squelch_stats* stats;         /* [n_channels] after the last batch, or NULL */
+} abg_replay_job;
+/* ABG_ERANGE for a bad dev or a window with a sample outside the history (the message gives the range needed), also when
+ * the history is off; ABG_EINVAL for n_jobs outside [1, 65535], a null jobs, a channel list abg_create refuses, n_batches < 1 and null
+ * waveout or axcindicate. */
+ABG_API int abg_history_replay(abg_engine* e, int n_jobs, const abg_replay_job* jobs);
+/* Measurement aid: device time of the most recent abg_history_replay: ms2[0] = its gathers, ms2[1] = its replay engine's
+ * runs (K1 start to end of run, summed over the chunks); 0 before the first. */
+ABG_API int abg_debug_replay_time(abg_engine* e, float* ms2);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

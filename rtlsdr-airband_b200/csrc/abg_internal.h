@@ -333,6 +333,16 @@ struct HiCapture {  // one capture launch: outputs [m0, m0 + n_out) of one devic
 };
 cudaError_t abg_launch_history_capture(HiCapture c, cudaStream_t s);
 
+// history replay (replay.cu): see abg_history_replay in include/airband_b200.h
+struct RpGather {  // one job's bytes of one chunk
+    const unsigned char* ring;       // the parent device's history ring: stream byte b at b mod ring_bytes
+    unsigned long long ring_bytes;   // a multiple of 16
+    unsigned long long src;          // stream byte of dst[0]
+    unsigned char* dst;              // raw[cur] + fill of the job's device in the replay engine, any alignment
+    unsigned long long n_bytes;      // 0 = none
+};
+cudaError_t abg_launch_replay_gather(const RpGather* jobs, int n_jobs, int blocks_per_job, cudaStream_t s);
+
 struct K2Launch {
     int G, Gp, P, wave_batch, fm_demod, iq_stride;  // iq_stride = nbmax * B
     int lanes_per_warp;       // channels handled by one warp of K2: 1, 2, 4, 8, 16 or 32

@@ -461,7 +461,7 @@ struct Group {
     DevBuf<long long> tc_sq;
     DevBuf<int32_t> tc_tab_of_dev;
     double tc_cscale = 0.0;
-    int tc_tables = 0;
+    int tc_tables = 0;  // tables the buffers have room for
 };
 
 struct Slot {
@@ -543,6 +543,24 @@ struct abg_engine {
     DevBuf<int32_t> mix_flags;  // [nbmax][n_mixers]
     std::deque<std::pair<int, int>> mix_ready;  // (slot, batch-in-run), same for every mixer
     std::vector<int> mix_fetched;               // per mixer: entries of mix_ready already popped by that mixer
+    // history replay (abg_history_replay): the replay engine, one device per job, and the gather's records; created by the
+    // first replay, kept while its shape fits, freed when the last history is switched off
+    bool replay_engine = false;       // this engine is one: K1 groups split by the path a one-device engine would take
+    struct ReplayDevice {  // one device of the replay engine: the shape it was built for and its latest channel list
+        int32_t sfmt = 0, sample_rate = 0;
+        float fullscale = 0.0f;
+        bool afc = false, iq = false;  // some channel has AFC / I/Q outputs
+        std::vector<abg_channel_cfg> chans;
+        bool same_shape(const ReplayDevice& o) const {
+            return sfmt == o.sfmt && sample_rate == o.sample_rate && memcmp(&fullscale, &o.fullscale, sizeof(float)) == 0 &&
+                   afc == o.afc && iq == o.iq && chans.size() == o.chans.size();
+        }
+    };
+    abg_engine* replay = nullptr;
+    std::vector<ReplayDevice> replay_pool;  // [replay->dev.size()]
+    DevBuf<RpGather> replay_gather;
+    cudaEvent_t replay_ev[2] = {nullptr, nullptr};  // gather start, gather end (the replay's K1 waits on it)
+    float replay_ms[2] = {0.0f, 0.0f};
 
     K2Launch k2_launch(int cur) const {
         K2Launch L{};
@@ -679,11 +697,26 @@ int monitor_fetch(abg_engine* e, MonitorLaunch<Cfg, Run, Dev>& m, int dev, int k
     return 1;
 }
 
+void engine_free(abg_engine* e);
+
+// The replay engine and the gather's records and events (abg_history_replay).
+void replay_free(abg_engine* e) {
+    if (e->replay) engine_free(e->replay);
+    e->replay = nullptr;
+    e->replay_pool.clear();
+    e->replay_gather.free();
+    for (auto& ev : e->replay_ev) {
+        if (ev) cudaEventDestroy(ev);
+        ev = nullptr;
+    }
+}
+
 void engine_free(abg_engine* e) {
     if (!e) return;
     cudaSetDevice(e->cuda_dev);
     if (e->stream) cudaStreamSynchronize(e->stream);
     if (e->stream_b) cudaStreamSynchronize(e->stream_b);
+    replay_free(e);
     for (auto& d : e->dev) {
         for (int i = 0; i < 2; i++)
             if (d.raw[i]) cudaFree(d.raw[i]);
@@ -845,7 +878,7 @@ int rebuild_tc_tables(abg_engine* e, Group& g) {
     for (size_t t = 0; t < nt; t++)
         abg_k1tc_build_table(g.tc, e->N, g.sfmt, g.h_wsc.data(), keys[t].data(), (int)keys[t].size(), tab.data() + t * g.tc.table_bytes,
                              sq.data() + t * g.tc.C2p, &g.tc_cscale);
-    if ((int)nt != g.tc_tables) {
+    if ((int)nt > g.tc_tables) {  // grow only: a smaller set of tables uses the front of the buffers
         g.tc_btab.free(); g.tc_sq.free();
         if (g.tc_btab.alloc(tab.size()) || g.tc_sq.alloc(sq.size())) return fail(ABG_ENOMEM, "Out of device memory for the tensor-core coefficient tables");
         g.tc_tables = (int)nt;
@@ -854,6 +887,106 @@ int rebuild_tc_tables(abg_engine* e, Group& g) {
     CU(cudaMemcpy(g.tc_btab.p, tab.data(), tab.size(), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(g.tc_sq.p, sq.data(), sizeof(long long) * sq.size(), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(g.tc_tab_of_dev.p, tab_of_dev.data(), sizeof(int32_t) * tab_of_dev.size(), cudaMemcpyHostToDevice));
+    return ABG_OK;
+}
+
+// The channels of cfg as parse_channels() resolves them (config.cpp:265-281,306-726): parameters, initial state, bins and
+// CTCSS banks of every channel into hp, hs, hb and h_coeff ([Gp] and [2][ABG_MAX_TONES][Gp]), and the engine flags that
+// follow from them.  The engine's devices are laid out already.  abg_create and every history replay start from it.
+// Which K1 a launch group of this format and hop takes, from its largest channel count and whether a device has AFC (a
+// group with AFC needs whole spectra): *use_tc with fft_mode 3, or 0 with tc_auto, when a tensor-core plan exists (into
+// *tc); *pruned unless fft_mode is 1 when the output-pruned kernel fits (its tile into *p_frames, *p_cap).  build() decides
+// every group with it, and a replay engine groups its devices by what it decides for each device alone.
+void k1_choice(const abg_engine* e, int sfmt, int hop_bytes, int max_channels, bool afc, bool* pruned, bool* use_tc, K1TcPlan* tc,
+               int* p_frames, int* p_cap) {
+    *p_frames = abg_k1p_tile_frames(e->N, sfmt, hop_bytes, max_channels, p_cap);
+    *pruned = (e->fft_mode != 1) && !afc && *p_frames >= 1;
+    const bool want_tc = e->fft_mode == 3 || (e->fft_mode == 0 && e->tc_auto);
+    *use_tc = want_tc && !afc && abg_k1tc_plan(e->N, sfmt, hop_bytes, max_channels, e->tc_digits, tc) == 1;
+}
+
+int resolve_channels(abg_engine* e, const abg_config* cfg, std::vector<ChanParams>& hp, std::vector<ChanState>& hs,
+                     std::vector<int32_t>& hb, std::vector<float>& h_coeff) {
+    const int N = e->N, G = e->G, Gp = e->Gp;
+    hp.assign(Gp, ChanParams{});
+    hs.assign(Gp, ChanState{});
+    hb.assign(Gp, 0);
+    h_coeff.assign((size_t)2 * ABG_MAX_TONES * Gp, 0.0f);
+    memset(hp.data(), 0, sizeof(ChanParams) * Gp);
+    memset(hs.data(), 0, sizeof(ChanState) * Gp);
+    e->any_iq_out = e->any_nfm = false;
+    for (int i = 0; i < cfg->n_devices; i++) {
+        const abg_device_cfg& dc = cfg->devices[i];
+        Device& d = e->dev[i];
+        d.has_afc = false;
+        for (int c = 0; c < dc.n_channels; c++) {
+            const abg_channel_cfg& cc = dc.channels[c];
+            const int g = d.g0 + c;
+            if (cc.bin < 0 || cc.bin >= N) return fail(ABG_EINVAL, "devices[%d].channels[%d]: bin %d outside 0..%d", i, c, cc.bin, N - 1);
+            ChanParams& p = hp[g];
+            ChanState& s = hs[g];
+            hb[g] = cc.bin;
+            p.dev = i;
+            p.needs_raw_iq = cc.needs_raw_iq ? 1 : 0;
+            p.has_iq_outputs = cc.has_iq_outputs ? 1 : 0;
+            if (p.has_iq_outputs) e->any_iq_out = true;
+            p.dm_dphi = cc.dm_dphi;
+            p.alpha = cc.alpha;
+            p.afc = cc.afc & 0xff;
+            if (p.afc) d.has_afc = true;
+            {
+                char what[64];
+                snprintf(what, sizeof(what), "devices[%d].channels[%d]", i, c);
+                std::vector<float> banks[2];
+                const int rc = build_freq(e->W, cc, p, s, banks, what);
+                if (rc != ABG_OK) return rc;
+                for (int w = 0; w < 2; w++)
+                    for (size_t t = 0; t < banks[w].size(); t++) h_coeff[((size_t)w * ABG_MAX_TONES + t) * Gp + g] = banks[w][t];
+            }
+            // ---- mk_freqlist / parse_channels initial values, config.cpp:265-281,313-331 ----
+            s.dm_phi = 0;
+            s.pr = s.pj = 0.0f;
+            s.prev_waveout = 0.5f;
+            s.axc_prev = ABG_NO_SIGNAL;
+        }
+    }
+    e->h_params = hp;
+    for (int g = 0; g < G; g++)
+        if (hp[g].modulation == ABG_MOD_NFM) e->any_nfm = true;
+    e->h_bins = hb;
+    return ABG_OK;
+}
+
+// Upload what resolve_channels built and reset every buffer K2 carries from batch to batch, the AGC look-back rows
+// primed: the channel state abg_create leaves behind.
+int upload_channels(abg_engine* e, const std::vector<ChanParams>& hp, const std::vector<ChanState>& hs, const std::vector<int32_t>& hb,
+                    const std::vector<float>& h_coeff) {
+    const int Gp = e->Gp, B = e->B;
+    const size_t PG = (size_t)e->P * Gp;
+    CU(cudaMemcpy(e->params.p, hp.data(), sizeof(ChanParams) * Gp, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(e->state.p, hs.data(), sizeof(ChanState) * Gp, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(e->bins.p, hb.data(), sizeof(int32_t) * Gp, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(e->base_bins.p, hb.data(), sizeof(int32_t) * Gp, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(e->tone_coeff.p, h_coeff.data(), sizeof(float) * h_coeff.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemset(e->tone_q1.p, 0, sizeof(float) * h_coeff.size()));
+    CU(cudaMemset(e->tone_q2.p, 0, sizeof(float) * h_coeff.size()));
+    CU(cudaMemset(e->tone_mag.p, 0, sizeof(float) * h_coeff.size()));
+    CU(cudaMemset(e->sqbuf.p, 0, sizeof(float) * ABG_SQ_BUF * Gp));  // calloc, squelch.cpp:70
+    CU(cudaMemset(e->iqin[0].p, 0, sizeof(float2) * PG));
+    CU(cudaMemset(e->iqin[1].p, 0, sizeof(float2) * PG));
+    if (e->any_iq_out) CU(cudaMemset(e->iqout.p, 0, sizeof(float2) * (size_t)Gp * e->nbmax * B));
+    {
+        // config.cpp:313-316: wavein[0..AGC_EXTRA) = 20, waveout[0..AGC_EXTRA) = 0.5.  (wavein's priming values are
+        // overwritten by the first AGC_EXTRA frames because waveend starts at 0, config.cpp:805; kept for fidelity.)
+        std::vector<float> hw(PG, 0.0f), ho(PG, 0.0f);
+        for (int k = 0; k < ABG_AGC_EXTRA; k++)
+            for (int g = 0; g < Gp; g++) hw[(size_t)k * Gp + g] = 20.0f;
+        for (int g = 0; g < Gp; g++)
+            for (int k = 0; k < ABG_AGC_EXTRA; k++) ho[(size_t)g * e->P + k] = 0.5f;
+        CU(cudaMemcpy(e->win[0].p, hw.data(), sizeof(float) * PG, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(e->win[1].p, hw.data(), sizeof(float) * PG, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(e->wout.p, ho.data(), sizeof(float) * PG, cudaMemcpyHostToDevice));
+    }
     return ABG_OK;
 }
 
@@ -904,51 +1037,12 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
     e->Gp = (G + 31) & ~31;
     const int Gp = e->Gp;
 
-    // ---- per-channel parameters and initial state ----------------------------------------------------------------
-    std::vector<ChanParams> hp(Gp);
-    std::vector<ChanState> hs(Gp);
-    std::vector<int32_t> hb(Gp, 0);
-    std::vector<float> h_coeff((size_t)2 * ABG_MAX_TONES * Gp, 0.0f);
-    memset(hp.data(), 0, sizeof(ChanParams) * Gp);
-    memset(hs.data(), 0, sizeof(ChanState) * Gp);
-    for (int i = 0; i < cfg->n_devices; i++) {
-        const abg_device_cfg& dc = cfg->devices[i];
-        Device& d = e->dev[i];
-        for (int c = 0; c < dc.n_channels; c++) {
-            const abg_channel_cfg& cc = dc.channels[c];
-            const int g = d.g0 + c;
-            if (cc.bin < 0 || cc.bin >= N) return fail(ABG_EINVAL, "devices[%d].channels[%d]: bin %d outside 0..%d", i, c, cc.bin, N - 1);
-            ChanParams& p = hp[g];
-            ChanState& s = hs[g];
-            hb[g] = cc.bin;
-            p.dev = i;
-            p.needs_raw_iq = cc.needs_raw_iq ? 1 : 0;
-            p.has_iq_outputs = cc.has_iq_outputs ? 1 : 0;
-            if (p.has_iq_outputs) e->any_iq_out = true;
-            p.dm_dphi = cc.dm_dphi;
-            p.alpha = cc.alpha;
-            p.afc = cc.afc & 0xff;
-            if (p.afc) d.has_afc = true;
-            {
-                char what[64];
-                snprintf(what, sizeof(what), "devices[%d].channels[%d]", i, c);
-                std::vector<float> banks[2];
-                const int rc = build_freq(e->W, cc, p, s, banks, what);
-                if (rc != ABG_OK) return rc;
-                for (int w = 0; w < 2; w++)
-                    for (size_t t = 0; t < banks[w].size(); t++) h_coeff[((size_t)w * ABG_MAX_TONES + t) * Gp + g] = banks[w][t];
-            }
-            // ---- mk_freqlist / parse_channels initial values, config.cpp:265-281,313-331 ----
-            s.dm_phi = 0;
-            s.pr = s.pj = 0.0f;
-            s.prev_waveout = 0.5f;
-            s.axc_prev = ABG_NO_SIGNAL;
-        }
-    }
-    e->h_params = hp;
-    for (int g = 0; g < G; g++)
-        if (hp[g].modulation == ABG_MOD_NFM) e->any_nfm = true;
-    e->h_bins = hb;
+    std::vector<ChanParams> hp;
+    std::vector<ChanState> hs;
+    std::vector<int32_t> hb;
+    std::vector<float> h_coeff;
+    int rc = resolve_channels(e, cfg, hp, hs, hb, h_coeff);  // per-channel parameters and initial state
+    if (rc != ABG_OK) return rc;
 
     // ---- tables -----------------------------------------------------------------------------------------------------
     const std::vector<float> window = make_window(N);
@@ -981,12 +1075,23 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
     }
 
     // ---- groups (one K1 launch per sample format / full-scale / hop) ------------------------------------------------------
+    // A replay engine also keeps devices apart whose one-device engines would take different K1 paths (below): the paths
+    // do not round alike, and a replayed job must be bitwise what such an engine computes.
+    auto alone_path = [&](const Device& d) {
+        if (!e->replay_engine) return 0;
+        bool pruned = false, use_tc = false;
+        K1TcPlan tc{};
+        int frames = 0, cap = 0;
+        k1_choice(e, d.sfmt, d.hop_bytes, d.C, d.has_afc, &pruned, &use_tc, &tc, &frames, &cap);
+        return use_tc ? 3 : pruned ? 2 : 1;
+    };
+    std::vector<int> group_path;
     for (int i = 0; i < (int)e->dev.size(); i++) {
         Device& d = e->dev[i];
         int gi = -1;
         for (int k = 0; k < (int)e->groups.size(); k++)
             if (e->groups[k].sfmt == d.sfmt && e->groups[k].hop_bytes == d.hop_bytes &&
-                (d.sfmt == ABG_SFMT_U8 || d.sfmt == ABG_SFMT_S8 || e->groups[k].fullscale == d.fullscale))
+                (d.sfmt == ABG_SFMT_U8 || d.sfmt == ABG_SFMT_S8 || e->groups[k].fullscale == d.fullscale) && group_path[k] == alone_path(d))
                 gi = k;
         if (gi < 0) {
             Group g;
@@ -994,6 +1099,7 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
             g.hop_bytes = d.hop_bytes;
             g.fullscale = d.fullscale;
             e->groups.push_back(g);
+            group_path.push_back(alone_path(d));
             gi = (int)e->groups.size() - 1;
         }
         d.group = gi;
@@ -1051,12 +1157,9 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
             g.max_channels = std::max(g.max_channels, e->dev[di].C);
             if (e->dev[di].has_afc) group_afc = true;
         }
-        g.p_frames_per_tile = abg_k1p_tile_frames(N, g.sfmt, g.hop_bytes, g.max_channels, &g.p_tile_bytes_cap);
         // fft_mode: 0 auto; 1 = full spectrum every frame; 2 = output-pruned last pass on the FP32 pipes; 3 = the bins' DFT as an
         // integer GEMM on the tensor cores (8-bit formats; other groups fall back to 2).  Groups with AFC need whole spectra.
-        g.pruned = (e->fft_mode != 1) && !group_afc && g.p_frames_per_tile >= 1;
-        const bool want_tc = e->fft_mode == 3 || (e->fft_mode == 0 && e->tc_auto);
-        g.use_tc = want_tc && !group_afc && abg_k1tc_plan(N, g.sfmt, g.hop_bytes, g.max_channels, e->tc_digits, &g.tc) == 1;
+        k1_choice(e, g.sfmt, g.hop_bytes, g.max_channels, group_afc, &g.pruned, &g.use_tc, &g.tc, &g.p_frames_per_tile, &g.p_tile_bytes_cap);
         const float scale = sample_scale(g.sfmt, g.fullscale);  // window * 1/full-scale
         std::vector<float> wsc(N);
         for (int i = 0; i < N; i++) wsc[i] = window[i] * scale;
@@ -1087,34 +1190,12 @@ int build(abg_engine* e, const abg_config* cfg, const abg_options* opt) {
         e->tw2.alloc(std::max<size_t>(h_tw2.size(), 1)) || e->twn.alloc(h_twn.size()) || e->axc.alloc((size_t)e->nbmax * Gp) ||
         (e->any_iq_out && e->iqout.alloc((size_t)Gp * e->nbmax * B)))
         return fail(ABG_ENOMEM, "Out of device memory. Try fewer devices per GPU or a smaller max_batches_per_run.");
-    CU(cudaMemcpy(e->params.p, hp.data(), sizeof(ChanParams) * Gp, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(e->state.p, hs.data(), sizeof(ChanState) * Gp, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(e->bins.p, hb.data(), sizeof(int32_t) * Gp, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(e->base_bins.p, hb.data(), sizeof(int32_t) * Gp, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(e->tone_coeff.p, h_coeff.data(), sizeof(float) * h_coeff.size(), cudaMemcpyHostToDevice));
-    CU(cudaMemset(e->tone_q1.p, 0, sizeof(float) * h_coeff.size()));
-    CU(cudaMemset(e->tone_q2.p, 0, sizeof(float) * h_coeff.size()));
-    CU(cudaMemset(e->tone_mag.p, 0, sizeof(float) * h_coeff.size()));
-    CU(cudaMemset(e->sqbuf.p, 0, sizeof(float) * ABG_SQ_BUF * Gp));  // calloc, squelch.cpp:70
     CU(cudaMemcpy(e->lut.p, h_lut.data(), sizeof(float) * h_lut.size(), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(e->tw1.p, h_tw1.data(), sizeof(float2) * h_tw1.size(), cudaMemcpyHostToDevice));
     if (!h_tw2.empty()) CU(cudaMemcpy(e->tw2.p, h_tw2.data(), sizeof(float2) * h_tw2.size(), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(e->twn.p, h_twn.data(), sizeof(float2) * h_twn.size(), cudaMemcpyHostToDevice));
-    CU(cudaMemset(e->iqin[0].p, 0, sizeof(float2) * PG));
-    CU(cudaMemset(e->iqin[1].p, 0, sizeof(float2) * PG));
-    if (e->any_iq_out) CU(cudaMemset(e->iqout.p, 0, sizeof(float2) * (size_t)Gp * e->nbmax * B));
-    {
-        // config.cpp:313-316: wavein[0..AGC_EXTRA) = 20, waveout[0..AGC_EXTRA) = 0.5.  (wavein's priming values are
-        // overwritten by the first AGC_EXTRA frames because waveend starts at 0, config.cpp:805; kept for fidelity.)
-        std::vector<float> hw(PG, 0.0f), ho(PG, 0.0f);
-        for (int k = 0; k < ABG_AGC_EXTRA; k++)
-            for (int g = 0; g < Gp; g++) hw[(size_t)k * Gp + g] = 20.0f;
-        for (int g = 0; g < Gp; g++)
-            for (int k = 0; k < ABG_AGC_EXTRA; k++) ho[(size_t)g * e->P + k] = 0.5f;
-        CU(cudaMemcpy(e->win[0].p, hw.data(), sizeof(float) * PG, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(e->win[1].p, hw.data(), sizeof(float) * PG, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(e->wout.p, ho.data(), sizeof(float) * PG, cudaMemcpyHostToDevice));
-    }
+    rc = upload_channels(e, hp, hs, hb, h_coeff);
+    if (rc != ABG_OK) return rc;
     CU(cudaMalloc((void**)&e->d_k2, sizeof(K2Dev) * e->dev.size() + 16));
     e->h_k2.assign(e->dev.size(), K2Dev{});
     e->slots.resize(3);
@@ -1436,17 +1517,45 @@ int enqueue_run(abg_engine* e, const std::vector<int>& nb, bool resident, bool q
     return ABG_OK;
 }
 
-}  // namespace
+// Room for nbytes more input of device dev at raw[cur] + fill, compacting the buffer first when they do not fit: what
+// abg_push does before its copy, and the history replay before its gather.
+int ingest_room(abg_engine* e, int dev, size_t nbytes, const char* fn) {
+    Device& d = e->dev[dev];
+    if (d.fill + nbytes > d.cap) {
+        // compact: move the unconsumed tail to the front of the other buffer.  Ingest runs on its own stream so that
+        // host->device copies overlap K1; the other buffer may still be read by the most recent K1, so wait for it.
+        // keep the copy 16-byte aligned on both sides; with a sub-band output on, keep its filter's history too
+        const size_t hist = (size_t)e->subband.dev[dev].hist * d.bpc;
+        const size_t keep_from = (d.consumed > hist ? d.consumed - hist : 0) & ~(size_t)15;
+        const size_t rem = d.fill - keep_from;
+        if (rem + nbytes > d.cap) {
+            return fail(ABG_EOVERFLOW, "%s: device %d input buffer overflow (%zu buffered + %zu new > %zu)", fn, dev, d.fill - d.consumed, nbytes, d.cap);
+        }
+        // the destination buffer was last read by a K1 launched before the previous compaction: with at least one run since
+        // then that is run_index-2 or older, so the copy overlaps the K1 that is reading the current buffer right now
+        // (the band spectrum, the input meter, the sub-band outputs, the activity detector and the I/Q history's append read
+        // the same bytes right after that K1: ev_raw follows the last of them)
+        if (d.runs_since_compaction >= 1) {
+            if (e->run_index >= 2) {
+                CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 2) & 1], 0));
+                if (e->ev_raw[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_raw[(e->run_index - 2) & 1], 0));
+            }
+        } else if (e->run_index >= 1) {
+            CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 1) & 1], 0));
+            if (e->ev_raw[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_raw[(e->run_index - 1) & 1], 0));
+        }
+        d.runs_since_compaction = 0;
+        CU(cudaMemcpyAsync(d.raw[d.cur ^ 1], d.raw[d.cur] + keep_from, rem, cudaMemcpyDeviceToDevice, e->stream_c));
+        d.cur ^= 1;
+        d.fill = rem;
+        d.consumed -= keep_from;
+        d.dropped += keep_from;
+    }
+    return ABG_OK;
+}
 
-// =========================================================================================================================
-// C ABI
-// =========================================================================================================================
-extern "C" {
-
-const char* abg_last_error(void) { return g_err.c_str(); }
-const char* abg_version(void) { return "airband-b200 0.1 (sm_90a)"; }
-
-int abg_create(const abg_config* cfg, const abg_options* opt, abg_engine** out) {
+// abg_create; a replay engine (abg_history_replay) splits its K1 groups by the path each device alone would take.
+int create_engine(const abg_config* cfg, const abg_options* opt, bool replay_engine, abg_engine** out) {
     if (!cfg || !out) return fail(ABG_EINVAL, "abg_create: null argument");
     *out = nullptr;
     int ndev = 0;
@@ -1454,6 +1563,7 @@ int abg_create(const abg_config* cfg, const abg_options* opt, abg_engine** out) 
     if (er != cudaSuccess || ndev < 1)
         return fail(ABG_ENODEV, "Unable to find a CUDA device (%s). This engine has no CPU fallback.", er == cudaSuccess ? "device count is 0" : cudaGetErrorString(er));
     abg_engine* e = new abg_engine();
+    e->replay_engine = replay_engine;
     if (opt && opt->cuda_device >= 0) {
         e->cuda_dev = opt->cuda_device;
         if (cudaSetDevice(e->cuda_dev) != cudaSuccess) {
@@ -1481,6 +1591,18 @@ int abg_create(const abg_config* cfg, const abg_options* opt, abg_engine** out) 
     return ABG_OK;
 }
 
+}  // namespace
+
+// =========================================================================================================================
+// C ABI
+// =========================================================================================================================
+extern "C" {
+
+const char* abg_last_error(void) { return g_err.c_str(); }
+const char* abg_version(void) { return "airband-b200 0.1 (sm_90a)"; }
+
+int abg_create(const abg_config* cfg, const abg_options* opt, abg_engine** out) { return create_engine(cfg, opt, false, out); }
+
 void abg_destroy(abg_engine* e) { engine_free(e); }
 int abg_wave_batch(const abg_engine* e) { return e->B; }
 int abg_hop(const abg_engine* e, int dev) { return (dev < 0 || dev >= (int)e->dev.size()) ? ABG_ERANGE : e->dev[dev].hop; }
@@ -1491,36 +1613,8 @@ int abg_push(abg_engine* e, int dev, const void* iq, size_t nbytes) {
     if (nbytes == 0) return ABG_OK;
     if (nbytes % d.bpc) return fail(ABG_EINVAL, "abg_push: %zu bytes is not a whole number of complex samples", nbytes);
     cudaSetDevice(e->cuda_dev);
-    if (d.fill + nbytes > d.cap) {
-        // compact: move the unconsumed tail to the front of the other buffer.  Ingest runs on its own stream so that
-        // host->device copies overlap K1; the other buffer may still be read by the most recent K1, so wait for it.
-        // keep the copy 16-byte aligned on both sides; with a sub-band output on, keep its filter's history too
-        const size_t hist = (size_t)e->subband.dev[dev].hist * d.bpc;
-        const size_t keep_from = (d.consumed > hist ? d.consumed - hist : 0) & ~(size_t)15;
-        const size_t rem = d.fill - keep_from;
-        if (rem + nbytes > d.cap) {
-            return fail(ABG_EOVERFLOW, "abg_push: device %d input buffer overflow (%zu buffered + %zu new > %zu)", dev, d.fill - d.consumed, nbytes, d.cap);
-        }
-        // the destination buffer was last read by a K1 launched before the previous compaction: with at least one run since
-        // then that is run_index-2 or older, so the copy overlaps the K1 that is reading the current buffer right now
-        // (the band spectrum, the input meter, the sub-band outputs, the activity detector and the I/Q history's append read
-        // the same bytes right after that K1: ev_raw follows the last of them)
-        if (d.runs_since_compaction >= 1) {
-            if (e->run_index >= 2) {
-                CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 2) & 1], 0));
-                if (e->ev_raw[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_raw[(e->run_index - 2) & 1], 0));
-            }
-        } else if (e->run_index >= 1) {
-            CU(cudaStreamWaitEvent(e->stream_c, e->ev_k1[(e->run_index - 1) & 1], 0));
-            if (e->ev_raw[0]) CU(cudaStreamWaitEvent(e->stream_c, e->ev_raw[(e->run_index - 1) & 1], 0));
-        }
-        d.runs_since_compaction = 0;
-        CU(cudaMemcpyAsync(d.raw[d.cur ^ 1], d.raw[d.cur] + keep_from, rem, cudaMemcpyDeviceToDevice, e->stream_c));
-        d.cur ^= 1;
-        d.fill = rem;
-        d.consumed -= keep_from;
-        d.dropped += keep_from;
-    }
+    const int rc = ingest_room(e, dev, nbytes, "abg_push");
+    if (rc != ABG_OK) return rc;
     CU(cudaMemcpyAsync(d.raw[d.cur] + d.fill, iq, nbytes, cudaMemcpyHostToDevice, e->stream_c));
     e->ingest_dirty = true;
     d.fill += nbytes;
@@ -2084,6 +2178,7 @@ int abg_history_configure(abg_engine* e, int dev, int n_batches) {
         c.ring_bytes = s.ring.n;
         return ABG_OK;
     });
+    if (e->history.devs.empty()) replay_free(e);  // nothing left to replay
     return rc != ABG_OK ? rc : rp;
 }
 
@@ -2175,6 +2270,201 @@ int abg_debug_history_time(abg_engine* e, float* ms2) {
     const int rc = monitor_time(e, e->history, ms2, __func__);
     if (rc != ABG_OK) return rc;
     ms2[1] = e->history.capture_ms;
+    return ABG_OK;
+}
+
+// ---- history replay (definition in airband_b200.h) ---------------------------------------------------------------------
+// The replay engine is a pool of devices, each built for one shape of job (format, full scale, sample rate, channel count,
+// AFC, I/Q outputs: what sizes its buffers and picks its K1 path).  A call takes, for every job, an unused pool device of
+// its shape; the others get no input and advance no further.  The pool only grows: it is rebuilt, with every device it
+// had plus one for each job that found none, only when a call needs more devices of a shape than it holds, because
+// freeing device memory waits for the whole GPU.  Otherwise the channels of every pool device are re-resolved (an idle
+// device keeps the last channel list it ran) and the state reset to what abg_create leaves.
+static int replay_reset(abg_engine* r, const abg_config* c) {
+    CU(cudaStreamSynchronize(r->stream_c));
+    CU(cudaStreamSynchronize(r->stream));
+    CU(cudaStreamSynchronize(r->stream_b));
+    std::vector<ChanParams> hp;
+    std::vector<ChanState> hs;
+    std::vector<int32_t> hb;
+    std::vector<float> h_coeff;
+    int rc = resolve_channels(r, c, hp, hs, hb, h_coeff);
+    if (rc != ABG_OK) return rc;
+    if ((rc = upload_channels(r, hp, hs, hb, h_coeff)) != ABG_OK) return rc;
+    for (auto& g : r->groups)
+        if (g.use_tc && (rc = rebuild_tc_tables(r, g)) != ABG_OK) return rc;
+    for (auto& d : r->dev) {
+        d.primed = false;
+        d.cur = 0;
+        d.fill = d.consumed = d.dropped = 0;
+        d.runs_since_compaction = 1;
+        d.ready.clear();
+        d.batch_seq = d.audio_seq = 0;
+    }
+    for (auto& s : r->slots) s.pending = 0;
+    // upload_channels writes on the legacy stream, which the engine's non-blocking streams are not ordered after
+    CU(cudaStreamSynchronize(0));
+    return ABG_OK;
+}
+
+int abg_history_replay(abg_engine* e, int n_jobs, const abg_replay_job* jobs) {
+    if (n_jobs < 1 || n_jobs > 65535 || !jobs) return fail(ABG_EINVAL, "abg_history_replay: %d jobs at %p (1 to 65535)", n_jobs, (const void*)jobs);
+    const int B = e->B, N = e->N;
+    std::vector<abg_engine::ReplayDevice> want(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const abg_replay_job& J = jobs[j];
+        const HiDev* h = monitor_dev(e, e->history, J.dev, __func__);
+        if (!h) return ABG_ERANGE;
+        if (J.n_batches < 1 || J.n_channels < 1 || !J.channels || !J.waveout || !J.axcindicate)
+            return fail(ABG_EINVAL, "abg_history_replay: job %d: %d batches of %d channels (%p) into waveout %p, axcindicate %p", j, J.n_batches,
+                        J.n_channels, (const void*)J.channels, (void*)J.waveout, (void*)J.axcindicate);
+        const Device& d = e->dev[J.dev];
+        // the samples the replay reads: from S to the end of its last frame, fft_size - hop into the batch after the last
+        const unsigned __int128 S = (unsigned __int128)J.first_batch * B * d.hop;
+        const unsigned __int128 end = S + (unsigned __int128)(ABG_AGC_EXTRA + (unsigned long long)J.n_batches * B) * d.hop + N - d.hop;
+        if (h->first == h->end || S < h->first || end > h->end)
+            return fail(ABG_ERANGE, "abg_history_replay: job %d reads samples [%llu, %llu) of device %d, outside its history [%llu, %llu)", j,
+                        (unsigned long long)S, (unsigned long long)end, J.dev, (unsigned long long)h->first, (unsigned long long)h->end);
+        // what abg_create refuses in a channel list, checked before the pool is touched
+        bool afc = false, iq = false;
+        for (int c = 0; c < J.n_channels; c++) {
+            const abg_channel_cfg& cc = J.channels[c];
+            char what[64];
+            snprintf(what, sizeof(what), "abg_history_replay: jobs[%d].channels[%d]", j, c);
+            if (cc.bin < 0 || cc.bin >= N) return fail(ABG_EINVAL, "%s: bin %d outside 0..%d", what, cc.bin, N - 1);
+            ChanParams p{};
+            ChanState st{};
+            std::vector<float> banks[2];
+            const int rc = build_freq(e->W, cc, p, st, banks, what);
+            if (rc != ABG_OK) return rc;
+            afc |= (cc.afc & 0xff) != 0;
+            iq |= cc.has_iq_outputs != 0;
+        }
+        abg_engine::ReplayDevice& w = want[j];
+        w.sfmt = d.sfmt;
+        w.fullscale = d.fullscale;
+        w.sample_rate = d.sample_rate;
+        w.afc = afc;
+        w.iq = iq;
+        w.chans.assign(J.channels, J.channels + J.n_channels);
+    }
+    // every job to an unused pool device of its shape; the pool grows by the jobs that find none
+    std::vector<abg_engine::ReplayDevice> pool = e->replay_pool;
+    std::vector<int> slot(n_jobs, -1);
+    std::vector<bool> used(pool.size(), false);
+    bool grow = !e->replay;
+    for (int j = 0; j < n_jobs; j++) {
+        for (size_t p = 0; p < pool.size() && slot[j] < 0; p++)
+            if (!used[p] && pool[p].same_shape(want[j])) {
+                slot[j] = (int)p;
+                used[p] = true;
+            }
+        if (slot[j] < 0) {
+            slot[j] = (int)pool.size();
+            pool.push_back(want[j]);
+            used.push_back(true);
+            grow = true;
+        }
+        pool[slot[j]].chans = want[j].chans;
+    }
+    std::vector<abg_device_cfg> devs(pool.size());
+    for (size_t p = 0; p < pool.size(); p++)
+        devs[p] = abg_device_cfg{pool[p].sfmt, pool[p].fullscale, pool[p].sample_rate, (int32_t)pool[p].chans.size(), pool[p].chans.data()};
+    const abg_config rc_cfg{N, e->W, e->fm_demod, (int32_t)pool.size(), devs.data()};
+    cudaSetDevice(e->cuda_dev);
+    int rc;
+    if (!grow) {
+        rc = replay_reset(e->replay, &rc_cfg);
+    } else {
+        if (e->replay) engine_free(e->replay);
+        e->replay = nullptr;
+        e->replay_pool.clear();
+        abg_options o{};
+        o.cuda_device = e->cuda_dev;
+        o.max_batches_per_run = e->nbmax;
+        o.fft_mode = e->fft_mode;
+        rc = create_engine(&rc_cfg, &o, true, &e->replay);
+        if (rc == ABG_OK && !e->replay_ev[0])
+            for (auto& ev : e->replay_ev) CU(cudaEventCreate(&ev));
+    }
+    if (rc != ABG_OK) return rc;
+    e->replay_pool = pool;
+    cudaSetDevice(e->cuda_dev);
+    // upload_small writes whole 16-byte words: one record of room for the rounding
+    if (e->replay_gather.n < (size_t)n_jobs + 1) {
+        e->replay_gather.free();
+        if (e->replay_gather.alloc((size_t)n_jobs + 1)) return fail(ABG_ENOMEM, "Out of device memory for the history replay");
+    }
+    abg_engine* r = e->replay;
+    std::vector<int> done(n_jobs, 0);                       // batches fetched
+    std::vector<unsigned long long> pushed(n_jobs, 0);      // bytes gathered
+    std::vector<RpGather> g(n_jobs);
+    float ms_gather = 0.0f, ms_run = 0.0f;
+    for (;;) {
+        // the chunk: up to max_batches_per_run more batches of every job (AFC devices advance one batch per run)
+        std::vector<int> nb(n_jobs, 0);
+        unsigned long long max_bytes = 0;
+        int total = 0;
+        for (int j = 0; j < n_jobs; j++) {
+            const abg_replay_job& J = jobs[j];
+            const Device& d = e->dev[J.dev];
+            const HiDev& h = e->history.dev[J.dev];
+            Device& rd = r->dev[slot[j]];
+            nb[j] = std::min(rd.has_afc ? 1 : r->nbmax, J.n_batches - done[j]);
+            g[j] = RpGather{h.ring.p, h.ring.n, J.first_batch * B * d.hop * d.bpc + pushed[j], nullptr, 0};
+            if (nb[j] == 0) continue;
+            // the bytes the fill rule needs for done + nb batches (rtl_airband.cpp:394-400)
+            const unsigned long long want_bytes = ((ABG_AGC_EXTRA + (unsigned long long)(done[j] + nb[j]) * B) * d.hop + N) * d.bpc;
+            const unsigned long long n = want_bytes - pushed[j];
+            if ((rc = ingest_room(r, slot[j], n, "abg_history_replay")) != ABG_OK) return rc;
+            g[j].dst = rd.raw[rd.cur] + rd.fill;
+            g[j].n_bytes = n;
+            rd.fill += n;
+            pushed[j] = want_bytes;
+            max_bytes = std::max(max_bytes, n);
+            total += nb[j];
+        }
+        if (total == 0) break;
+        // the gather on the K1 stream: behind every append it reads, ahead of every later one that would overwrite them
+        const int nl = upload_small(e->replay_gather.p, g.data(), sizeof(RpGather) * n_jobs, e->stream);
+        if (nl < 0) return fail(ABG_ECUDA, "history replay parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+        e->launches += (uint64_t)nl;
+        CU(cudaEventRecord(e->replay_ev[0], e->stream));
+        const cudaError_t er = abg_launch_replay_gather(e->replay_gather.p, n_jobs, abg_history_blocks(max_bytes, n_jobs, e->sm_count), e->stream);
+        if (er != cudaSuccess) return fail(ABG_ECUDA, "history replay gather launch failed: %s", cudaGetErrorString(er));
+        e->launches++;
+        CU(cudaEventRecord(e->replay_ev[1], e->stream));
+        CU(cudaStreamWaitEvent(r->stream, e->replay_ev[1], 0));
+        r->ingest_dirty = true;  // and behind any compaction on the replay engine's ingest stream
+        const int ran = abg_run(r, -1);
+        if (ran < 0) return ran;
+        if (ran != total) return fail(ABG_ECUDA, "abg_history_replay: the replay engine ran %d of %d batches", ran, total);
+        for (int j = 0; j < n_jobs; j++) {
+            const abg_replay_job& J = jobs[j];
+            const size_t C = (size_t)J.n_channels, o = (size_t)done[j];
+            const int got = abg_fetch_batches(r, slot[j], nb[j], J.waveout + o * C * B, J.iq_out ? J.iq_out + o * C * 2 * B : nullptr,
+                                              J.axcindicate + o * C);
+            if (got < 0) return got;
+            done[j] += got;
+        }
+        float ms = 0.0f, ms4[4];
+        CU(cudaEventElapsedTime(&ms, e->replay_ev[0], e->replay_ev[1]));
+        if ((rc = abg_last_run_times(r, ms4)) != ABG_OK) return rc;
+        ms_gather += ms;
+        ms_run += ms4[3];
+    }
+    for (int j = 0; j < n_jobs; j++)
+        for (int c = 0; jobs[j].stats && c < jobs[j].n_channels; c++)
+            if ((rc = abg_get_stats(r, slot[j], c, jobs[j].stats + c)) != ABG_OK) return rc;
+    e->replay_ms[0] = ms_gather;
+    e->replay_ms[1] = ms_run;
+    return ABG_OK;
+}
+
+int abg_debug_replay_time(abg_engine* e, float* ms2) {
+    if (!ms2) return fail(ABG_EINVAL, "abg_debug_replay_time: null argument");
+    ms2[0] = e->replay_ms[0];
+    ms2[1] = e->replay_ms[1];
     return ABG_OK;
 }
 

@@ -11,7 +11,7 @@ from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .config import AGC_EXTRA, CConfig, CSquelchStats, Config
+from .config import AGC_EXTRA, CChannelCfg, CConfig, CSquelchStats, Config, channels_to_c, make_channel
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_DIR = os.path.abspath(os.path.join(_HERE, "..", ".."))
@@ -30,6 +30,7 @@ SYMBOLS = [
     "abg_tone_meter_configure", "abg_tone_meter_set_tones", "abg_fetch_tone_meter", "abg_debug_tone_meter_time",
     "abg_activity_configure", "abg_fetch_activity", "abg_debug_activity_time",
     "abg_history_configure", "abg_history_range", "abg_history_raw", "abg_history_subband", "abg_debug_history_time",
+    "abg_history_replay", "abg_debug_replay_time",
 ]
 
 SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
@@ -82,6 +83,21 @@ class CBurst(C.Structure):
         ("peak", C.c_float),
         ("sum", C.c_float),
         ("reserved", C.c_int32),
+    ]
+
+
+class CReplayJob(C.Structure):
+    """abg_replay_job: one history replay job (definition in airband_b200.h)."""
+    _fields_ = [
+        ("dev", C.c_int32),
+        ("n_batches", C.c_int32),
+        ("first_batch", C.c_uint64),
+        ("n_channels", C.c_int32),
+        ("channels", C.POINTER(CChannelCfg)),
+        ("waveout", C.c_void_p),
+        ("iq_out", C.c_void_p),
+        ("axcindicate", C.c_void_p),
+        ("stats", C.POINTER(CSquelchStats)),
     ]
 
 
@@ -178,6 +194,8 @@ def load():
     L.abg_history_subband.restype = i
     L.abg_history_subband.argtypes = [vp, i, C.c_double, i, i, vp, C.c_uint64, C.c_int64, vp]
     L.abg_debug_history_time.restype, L.abg_debug_history_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_history_replay.restype, L.abg_history_replay.argtypes = i, [vp, i, C.POINTER(CReplayJob)]
+    L.abg_debug_replay_time.restype, L.abg_debug_replay_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -539,6 +557,36 @@ class Engine:
         stream; 0 where there was none."""
         ms = (C.c_float * 2)()
         self._chk(self.L.abg_debug_history_time(self.h, ms))
+        return float(ms[0]), float(ms[1])
+
+    def history_replay(self, jobs, want_iq: bool = True) -> List[dict]:
+        """Demodulate stretches of the history as fresh channels listening there would have (definition in
+        airband_b200.h), all jobs in one call.  jobs: dicts with dev, first_batch, n_batches and channels (a list of
+        config.Channel), e.g. from transmission_replay.  Returns per job a dict with waveout float32[n_batches, C, B],
+        iq complex64[n_batches, C, B] (None unless want_iq), axc uint8[n_batches, C] and stats (a CSquelchStats per
+        channel after the last batch)."""
+        arr = (CReplayJob * max(len(jobs), 1))()
+        keep, out = [], []
+        for k, j in enumerate(jobs):
+            chans = channels_to_c(j["channels"])
+            nb, Cn = int(j["n_batches"]), len(j["channels"])
+            r = dict(waveout=np.zeros((max(nb, 0), Cn, self.B), np.float32),
+                     iq=np.zeros((max(nb, 0), Cn, 2 * self.B), np.float32) if want_iq else None,
+                     axc=np.zeros((max(nb, 0), Cn), np.uint8), stats=(CSquelchStats * max(Cn, 1))())
+            keep.append(chans)
+            arr[k] = CReplayJob(int(j["dev"]), nb, int(j["first_batch"]), Cn, C.cast(chans, C.POINTER(CChannelCfg)),
+                                _ptr(r["waveout"]), _ptr(r["iq"]), _ptr(r["axc"]), C.cast(r["stats"], C.POINTER(CSquelchStats)))
+            out.append(r)
+        self._chk(self.L.abg_history_replay(self.h, len(jobs), arr))
+        for r in out:
+            r["iq"] = r["iq"].view(np.complex64) if r["iq"] is not None else None
+            r["stats"] = list(r["stats"])[:r["waveout"].shape[1]]
+        return out
+
+    def replay_time(self) -> Tuple[float, float]:
+        """(gather ms, replay engine run ms) of the most recent history_replay, from CUDA events; 0 before the first."""
+        ms = (C.c_float * 2)()
+        self._chk(self.L.abg_debug_replay_time(self.h, ms))
         return float(ms[0]), float(ms[1])
 
     # ---- mixers ---------------------------------------------------------------------------------------------------
@@ -928,3 +976,41 @@ def transmission_capture(tx: dict, cfg: Config, dev: int, history_range: Tuple[i
         raise ValueError(f"transmission_capture: nothing of the transmission (samples [{lo}, {hi})) is left in the history "
                          f"[{first}, {end}) with {L} taps at decimation {D}")
     return float(tx["freq_hz"]) - float(d.centerfreq), m_lo, m_hi - m_lo
+
+
+# A fresh AM channel's auto squelch starts from a noise floor of 5.0.  On the test signals' noise (U8 at 2.048 Msps, fft
+# 2048, complex noise of 0.01 full scale per component) the CPU oracle's noise level is within 10 % of its steady value
+# from the 6th batch on (tests/test_history_replay_cpu.py measures it): 6 batches of lead-in.
+REPLAY_SETTLE_BATCHES = 6
+
+
+def transmission_replay(tx: dict, cfg: Config, dev: int, history_range: Tuple[int, int], lead_s: Optional[float] = None,
+                        **channel_kw) -> dict:
+    """An Engine.history_replay job that listens to one transmission (a group_transmissions dict of device dev): a channel
+    from config.make_channel at tx["freq_hz"] (its bin, and dm_dphi for NFM; channel_kw goes to make_channel, e.g.
+    modulation, bandwidth, ctcss_hz).  first_batch is the latest batch whose first frame lies at least lead_s seconds of
+    frames before the transmission's first frame, or the first batch whose samples the history holds if that is later;
+    n_batches runs to the batch of its last frame, or as far as the history reaches: every sample read,
+    [first_batch * B * hop, (AGC_EXTRA + (first_batch + n_batches) * B) * hop + fft_size - hop), lies in history_range.
+    lead_s defaults to REPLAY_SETTLE_BATCHES batches (0.75 s at wave_rate 8000): the time a fresh channel's squelch takes
+    to find the noise floor, so that the transmission opens it as a configured channel's would.  Raises ValueError if
+    nothing of the transmission fits."""
+    d = cfg.devices[dev]
+    B, hop, N = cfg.wave_batch, cfg.hop(dev), cfg.fft_size
+    if lead_s is None:
+        lead_s = REPLAY_SETTLE_BATCHES * B / cfg.wave_rate
+    if lead_s < 0:
+        raise ValueError("transmission_replay: lead_s must be >= 0")
+    first, end = history_range
+    lead = int(np.ceil(lead_s * d.sample_rate / hop))  # frames
+    b_lead = (int(tx["first_frame"]) - AGC_EXTRA - lead) // B
+    b_first = -(-int(first) // (B * hop))
+    b0 = max(b_lead, b_first, 0)
+    b_last = (int(tx["last_frame"]) - AGC_EXTRA) // B
+    b_end = ((int(end) - N + hop) // hop - AGC_EXTRA) // B  # batches b < b_end have every sample in the history
+    n = min(b_last + 1, b_end) - b0
+    if end <= first or n < 1:
+        raise ValueError(f"transmission_replay: nothing of the transmission (frames [{tx['first_frame']}, {tx['last_frame']}]) fits "
+                         f"the history [{first}, {end}) with {lead_s} s of lead-in")
+    ch = make_channel(int(round(tx["freq_hz"])), d.centerfreq, d.sample_rate, N, cfg.wave_rate, **channel_kw)
+    return dict(dev=dev, first_batch=b0, n_batches=n, channels=[ch])
