@@ -553,6 +553,71 @@ ABG_API int abg_history_replay(abg_engine* e, int n_jobs, const abg_replay_job* 
  * runs (K1 start to end of run, summed over the chunks); 0 before the first. */
 ABG_API int abg_debug_replay_time(abg_engine* e, float* ms2);
 
+/* Live follow (not part of the reference surface: many transmissions the activity detector reports are still going when
+ * they are found, and a replay job stops at the history's end).  A follow session is the streaming form of a replay job:
+ * it is opened with a job's dev, first_batch and channels but no n_batches, and every abg_follow_run advances it over what
+ * the history has gained since, with its channel state carried over.
+ *   Output: batch b >= first_batch of a session (waveout, iq_out, axcindicate) is bitwise batch b - first_batch of
+ *     abg_history_replay on the job {dev, first_batch, n_batches >= b - first_batch + 1, channels}, and abg_follow_stats
+ *     after batch b is that job's stats.  It does not depend on how abg_follow_run calls split the batches, on
+ *     max_batches_per_run or the push pattern, on other sessions opening, closing, advancing or falling behind, or on
+ *     abg_history_replay calls in between.
+ *   Availability: batch b can be demodulated once the history holds every sample the replay reads for it, i.e. end >=
+ *     (AGC_EXTRA + (b+1)*WAVE_BATCH)*hop + fft_size - hop, while history batch L ends at (AGC_EXTRA + (L+1)*WAVE_BATCH)*hop.
+ *     Where WAVE_BATCH*hop >= fft_size - hop a session therefore trails the live engine by one batch at most (125 ms at
+ *     wave_rate 8000): after abg_follow_run its next_batch is the live engine's last batch L (L + 1 when fft_size <= hop).
+ *     abg_create also accepts configurations without it (fft_size 8192 with hop <= 8 at WAVE_BATCH 1000, for one); there
+ *     a session trails by ceil((fft_size - hop) / (WAVE_BATCH*hop)) batches.
+ *   Lost: once the history overwrites the session's next sample not yet read, the session is lost: its queued batches
+ *     stay fetchable, then abg_follow_fetch returns ABG_ERANGE.  A session falls behind when its queue is full or when
+ *     abg_follow_run is not called often enough.
+ *   Queue: a session holds at most queue_batches unfetched batches (enqueued or finished).  abg_follow_run advances it
+ *     only into free room, so an unfetched session stops; it does not stall other sessions or hold result slots they need.
+ * Computed on the GPU: private follow engines on the same CUDA device, built like the replay engine and kept apart from
+ * it, each a pool of devices built for one session shape; sessions in one engine share every K1 and K2 launch.  An engine
+ * is never rebuilt: a closed session's device goes back to the pool and is reset for the next session of its shape.  Per
+ * chunk of max_batches_per_run batches (one with AFC), abg_follow_run enqueues one gather kernel on the K1 stream (behind
+ * every append it reads, ahead of every later one that would overwrite them) and one run per follow engine with work; it
+ * decides availability and loss on the host from the enqueued history range and never waits for the live engine's work.
+ * Finished batches move from the follow engines' result slots into the sessions' queues at a later abg_follow_run or at
+ * the fetch that needs them.  Nothing is allocated before the first open; the follow engines are freed when the last
+ * history is switched off (abg_history_configure refuses any change to a device with open sessions) and by abg_destroy.
+ * The live engine's channels, outputs and runs are unaffected.  Scan mode does not apply to followed channels. */
+typedef struct abg_follow_status {
+    int32_t dev;          /* device whose history the session follows */
+    int32_t n_channels;
+    uint64_t next_batch;  /* the next batch abg_follow_run enqueues */
+    int32_t queued;       /* batches enqueued and not fetched yet: [next_batch - queued, next_batch) */
+    int32_t lost;         /* 1 once the history overwrote a sample the session still needed */
+} abg_follow_status;
+/* Open a session on dev from batch first_batch; *session receives its id (ids are never reused within an engine's
+ * lifetime).  first_batch may lie beyond the live edge: the session then waits until its samples arrive.  ABG_EINVAL for
+ * a channel list abg_create refuses, queue_batches < 1 and null arguments; ABG_ERANGE for a bad dev, a device whose
+ * history is off, and a start sample first_batch * WAVE_BATCH * hop below abg_history_range's first (the message gives
+ * the range).  Checks everything before any engine state is touched; may wait for the follow engines. */
+ABG_API int abg_follow_open(abg_engine* e, int dev, uint64_t first_batch, int n_channels, const abg_channel_cfg* channels,
+                            int queue_batches, int32_t* session);
+/* Close a session: its unfetched batches are dropped.  ABG_ERANGE for an unknown or closed id. */
+ABG_API int abg_follow_close(abg_engine* e, int32_t session);
+/* Advance every open session by up to max_batches batches (< 0: as far as the history and its queue room allow, over as
+ * many chunks as needed); returns the session-batches enqueued.  Does not wait for the live engine's work; a call that
+ * enqueues more than three chunks for one follow engine waits for that engine's run three chunks back. */
+ABG_API int abg_follow_run(abg_engine* e, int max_batches);
+/* Pop up to max_batches of a session's oldest batches into waveout[n][n_channels][WAVE_BATCH], iq_out[n][n_channels]
+ * [2*WAVE_BATCH] (may be NULL) and axcindicate[n][n_channels]; *first_batch (may be NULL) = the batch number of the first
+ * popped.  Returns the number popped, 0 if none is queued; waits for the runs that compute them.  ABG_ERANGE for an
+ * unknown id and for a lost session with nothing left queued; ABG_EINVAL for max_batches < 0 and null outputs. */
+ABG_API int abg_follow_fetch(abg_engine* e, int32_t session, int max_batches, float* waveout, float* iq_out, char* axcindicate,
+                             uint64_t* first_batch);
+/* A session's device, channel count, next batch, queued batches and lost flag.  Does not wait. */
+ABG_API int abg_follow_info(abg_engine* e, int32_t session, abg_follow_status* out);
+/* Squelch statistics of channel chan of a session after its batch next_batch - 1, as abg_get_stats gives them; waits for
+ * it.  ABG_ERANGE for an unknown id or a bad channel index, ABG_EINVAL for a null out. */
+ABG_API int abg_follow_stats(abg_engine* e, int32_t session, int chan, abg_squelch_stats* out);
+/* Measurement aid: device time of the most recent abg_follow_run: ms2[0] = its gathers, ms2[1] = its follow-engine runs
+ * (from the end of the chunk's gather to the end of the run, summed); 0 if it enqueued nothing.  Waits for them. */
+ABG_API int abg_debug_follow_time(abg_engine* e, float* ms2);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

@@ -18,9 +18,12 @@
 #include <string.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
+#include <cstdint>
 #include <complex>
 #include <deque>
+#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -561,6 +564,33 @@ struct abg_engine {
     DevBuf<RpGather> replay_gather;
     cudaEvent_t replay_ev[2] = {nullptr, nullptr};  // gather start, gather end (the replay's K1 waits on it)
     float replay_ms[2] = {0.0f, 0.0f};
+    // live follow (abg_follow_open ...): follow engines, each a pool of devices built for one session shape, and the open
+    // sessions; created by the first open, kept while a history is on, never rebuilt
+    struct FollowBatch {
+        std::vector<float> wout, iq;  // [C][B], [C][2B]
+        std::vector<char> axc;        // [C]
+    };
+    struct FollowSession {
+        int dev = 0, eng = 0, slot = 0;        // parent device; follow engine and its device
+        int C = 0, queue_batches = 0;
+        uint64_t first_batch = 0, next_batch = 0;  // next_batch: the next batch to enqueue
+        unsigned long long pushed = 0, valid = 0;  // bytes of the window in the follow device's buffer / gathered from the history
+        bool lost = false;
+        std::deque<FollowBatch> q;  // finished batches moved out of the follow engine's result slots, oldest first
+    };
+    struct FollowEngine {
+        abg_engine* r = nullptr;
+        std::vector<ReplayDevice> pool;  // [r->dev.size()]
+        std::vector<int32_t> owner;      // session id per device, -1 = free
+        cudaEvent_t ev_compact = nullptr;  // after the compactions of a chunk on r's ingest stream
+    };
+    std::vector<FollowEngine> follow;
+    std::map<int32_t, FollowSession> sessions;
+    int32_t next_session = 0;
+    DevBuf<RpGather> follow_gather;
+    std::vector<cudaEvent_t> follow_tev;  // (start, end) pairs: the latest abg_follow_run's gathers and runs
+    std::vector<int> follow_kind;         // per pair: 0 = gather, 1 = follow-engine run
+    int follow_pairs = 0;
 
     K2Launch k2_launch(int cur) const {
         K2Launch L{};
@@ -711,12 +741,28 @@ void replay_free(abg_engine* e) {
     }
 }
 
+// The follow engines, every session and the follow gather's records and events (abg_follow_open ...).
+void follow_free(abg_engine* e) {
+    for (auto& f : e->follow) {
+        engine_free(f.r);
+        if (f.ev_compact) cudaEventDestroy(f.ev_compact);
+    }
+    e->follow.clear();
+    e->sessions.clear();
+    e->follow_gather.free();
+    for (auto ev : e->follow_tev) cudaEventDestroy(ev);
+    e->follow_tev.clear();
+    e->follow_kind.clear();
+    e->follow_pairs = 0;
+}
+
 void engine_free(abg_engine* e) {
     if (!e) return;
     cudaSetDevice(e->cuda_dev);
     if (e->stream) cudaStreamSynchronize(e->stream);
     if (e->stream_b) cudaStreamSynchronize(e->stream_b);
     replay_free(e);
+    follow_free(e);
     for (auto& d : e->dev) {
         for (int i = 0; i < 2; i++)
             if (d.raw[i]) cudaFree(d.raw[i]);
@@ -2157,6 +2203,10 @@ int abg_history_configure(abg_engine* e, int dev, int n_batches) {
     if (!h) return ABG_ERANGE;
     if (n_batches < 0) return fail(ABG_EINVAL, "abg_history_configure: n_batches %d is negative", n_batches);
     if (n_batches == h->batches) return ABG_OK;
+    // a change of capacity empties the history under the device's follow sessions
+    for (const auto& s : e->sessions)
+        if (s.second.dev == dev)
+            return fail(ABG_EINVAL, "abg_history_configure: device %d has open follow sessions (session %d)", dev, (int)s.first);
     int rc = monitor_configure(e, e->history, n_batches > 0);  // an enqueued append or capture may still use the ring
     if (rc != ABG_OK) return rc;
     const Device& d = e->dev[dev];
@@ -2178,7 +2228,10 @@ int abg_history_configure(abg_engine* e, int dev, int n_batches) {
         c.ring_bytes = s.ring.n;
         return ABG_OK;
     });
-    if (e->history.devs.empty()) replay_free(e);  // nothing left to replay
+    if (e->history.devs.empty()) {  // nothing left to replay or follow (no session is open: see above)
+        replay_free(e);
+        follow_free(e);
+    }
     return rc != ABG_OK ? rc : rp;
 }
 
@@ -2307,6 +2360,34 @@ static int replay_reset(abg_engine* r, const abg_config* c) {
     return ABG_OK;
 }
 
+// The pool-device shape of a channel list for device d, after checking what abg_create refuses in it (`who` names the
+// list in errors): replay jobs and follow sessions check their lists with it before any engine state is touched.
+static int channel_shape(const abg_engine* e, const Device& d, int n_channels, const abg_channel_cfg* channels, const char* who,
+                         abg_engine::ReplayDevice* w) {
+    const int N = e->N;
+    bool afc = false, iq = false;
+    for (int c = 0; c < n_channels; c++) {
+        const abg_channel_cfg& cc = channels[c];
+        char what[96];
+        snprintf(what, sizeof(what), "%s.channels[%d]", who, c);
+        if (cc.bin < 0 || cc.bin >= N) return fail(ABG_EINVAL, "%s: bin %d outside 0..%d", what, cc.bin, N - 1);
+        ChanParams p{};
+        ChanState st{};
+        std::vector<float> banks[2];
+        const int rc = build_freq(e->W, cc, p, st, banks, what);
+        if (rc != ABG_OK) return rc;
+        afc |= (cc.afc & 0xff) != 0;
+        iq |= cc.has_iq_outputs != 0;
+    }
+    w->sfmt = d.sfmt;
+    w->fullscale = d.fullscale;
+    w->sample_rate = d.sample_rate;
+    w->afc = afc;
+    w->iq = iq;
+    w->chans.assign(channels, channels + n_channels);
+    return ABG_OK;
+}
+
 int abg_history_replay(abg_engine* e, int n_jobs, const abg_replay_job* jobs) {
     if (n_jobs < 1 || n_jobs > 65535 || !jobs) return fail(ABG_EINVAL, "abg_history_replay: %d jobs at %p (1 to 65535)", n_jobs, (const void*)jobs);
     const int B = e->B, N = e->N;
@@ -2325,28 +2406,10 @@ int abg_history_replay(abg_engine* e, int n_jobs, const abg_replay_job* jobs) {
         if (h->first == h->end || S < h->first || end > h->end)
             return fail(ABG_ERANGE, "abg_history_replay: job %d reads samples [%llu, %llu) of device %d, outside its history [%llu, %llu)", j,
                         (unsigned long long)S, (unsigned long long)end, J.dev, (unsigned long long)h->first, (unsigned long long)h->end);
-        // what abg_create refuses in a channel list, checked before the pool is touched
-        bool afc = false, iq = false;
-        for (int c = 0; c < J.n_channels; c++) {
-            const abg_channel_cfg& cc = J.channels[c];
-            char what[64];
-            snprintf(what, sizeof(what), "abg_history_replay: jobs[%d].channels[%d]", j, c);
-            if (cc.bin < 0 || cc.bin >= N) return fail(ABG_EINVAL, "%s: bin %d outside 0..%d", what, cc.bin, N - 1);
-            ChanParams p{};
-            ChanState st{};
-            std::vector<float> banks[2];
-            const int rc = build_freq(e->W, cc, p, st, banks, what);
-            if (rc != ABG_OK) return rc;
-            afc |= (cc.afc & 0xff) != 0;
-            iq |= cc.has_iq_outputs != 0;
-        }
-        abg_engine::ReplayDevice& w = want[j];
-        w.sfmt = d.sfmt;
-        w.fullscale = d.fullscale;
-        w.sample_rate = d.sample_rate;
-        w.afc = afc;
-        w.iq = iq;
-        w.chans.assign(J.channels, J.channels + J.n_channels);
+        char who[48];
+        snprintf(who, sizeof(who), "abg_history_replay: jobs[%d]", j);
+        const int rc = channel_shape(e, d, J.n_channels, J.channels, who, &want[j]);
+        if (rc != ABG_OK) return rc;
     }
     // every job to an unused pool device of its shape; the pool grows by the jobs that find none
     std::vector<abg_engine::ReplayDevice> pool = e->replay_pool;
@@ -2465,6 +2528,351 @@ int abg_debug_replay_time(abg_engine* e, float* ms2) {
     if (!ms2) return fail(ABG_EINVAL, "abg_debug_replay_time: null argument");
     ms2[0] = e->replay_ms[0];
     ms2[1] = e->replay_ms[1];
+    return ABG_OK;
+}
+
+// ---- live follow (definition in airband_b200.h) -------------------------------------------------------------------------
+// A session is a replay job without an end, on a device of its own in a follow engine: a private engine built like the
+// replay engine (K1 groups split by the path a one-device engine takes), kept apart from it because replay_reset resets
+// every device of its pool.  A follow engine is never rebuilt, since that would have to carry every open session's channel
+// state across layouts.  A closed session's device goes back to the pool, and the next session of its shape resets only
+// that device (follow_reset); a session that finds no free device of its shape gets a new engine with as many devices of
+// that shape as exist already, so the number of engines grows logarithmically.
+static abg_engine::FollowSession* follow_session(abg_engine* e, int32_t id, const char* fn) {
+    const auto it = e->sessions.find(id);
+    if (it != e->sessions.end()) return &it->second;
+    fail(ABG_ERANGE, "%s: no open follow session %d", fn, (int)id);
+    return nullptr;
+}
+
+// Device p of follow engine f back to the state a fresh engine with the channel list f.pool[p].chans leaves it in, its
+// neighbours untouched: parameters, state, bins and CTCSS banks of its channels, their tone-bank and Squelch delay-line
+// columns, their look-back rows in both run parities, its group's tensor-core tables and its ingest bookkeeping.
+static int follow_reset(abg_engine::FollowEngine& f, int p) {
+    abg_engine* r = f.r;
+    CU(cudaStreamSynchronize(r->stream_c));
+    CU(cudaStreamSynchronize(r->stream));
+    CU(cudaStreamSynchronize(r->stream_b));
+    std::vector<abg_device_cfg> devs(f.pool.size());
+    for (size_t k = 0; k < f.pool.size(); k++)
+        devs[k] = abg_device_cfg{f.pool[k].sfmt, f.pool[k].fullscale, f.pool[k].sample_rate, (int32_t)f.pool[k].chans.size(), f.pool[k].chans.data()};
+    const abg_config cfg{r->N, r->W, r->fm_demod, (int32_t)devs.size(), devs.data()};
+    std::vector<ChanParams> hp;
+    std::vector<ChanState> hs;
+    std::vector<int32_t> hb;
+    std::vector<float> hc;
+    int rc = resolve_channels(r, &cfg, hp, hs, hb, hc);  // the other devices resolve to the lists they were opened with
+    if (rc != ABG_OK) return rc;
+    Device& d = r->dev[p];
+    const int g0 = d.g0, C = d.C, Gp = r->Gp, P = r->P;
+    const size_t row = sizeof(float) * Gp, cols = sizeof(float) * C;
+    CU(cudaMemcpy(r->params.p + g0, hp.data() + g0, sizeof(ChanParams) * C, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(r->state.p + g0, hs.data() + g0, sizeof(ChanState) * C, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(r->bins.p + g0, hb.data() + g0, sizeof(int32_t) * C, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(r->base_bins.p + g0, hb.data() + g0, sizeof(int32_t) * C, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy2D(r->tone_coeff.p + g0, row, hc.data() + g0, row, cols, 2 * ABG_MAX_TONES, cudaMemcpyHostToDevice));
+    for (DevBuf<float>* t : {&r->tone_q1, &r->tone_q2, &r->tone_mag}) CU(cudaMemset2D(t->p + g0, row, 0, cols, 2 * ABG_MAX_TONES));
+    CU(cudaMemset2D(r->sqbuf.p + g0, row, 0, cols, ABG_SQ_BUF));
+    // the AGC look-back rows as upload_channels primes them: win [P][Gp] time-major, wout [Gp][P] channel-major
+    std::vector<float> hw((size_t)P * C, 0.0f), ho((size_t)C * P, 0.0f);
+    for (int k = 0; k < ABG_AGC_EXTRA; k++)
+        for (int c = 0; c < C; c++) {
+            hw[(size_t)k * C + c] = 20.0f;
+            ho[(size_t)c * P + k] = 0.5f;
+        }
+    for (int k = 0; k < 2; k++) {
+        CU(cudaMemcpy2D(r->win[k].p + g0, row, hw.data(), cols, cols, P, cudaMemcpyHostToDevice));
+        CU(cudaMemset2D(r->iqin[k].p + g0, sizeof(float2) * Gp, 0, sizeof(float2) * C, P));
+    }
+    CU(cudaMemcpy(r->wout.p + (size_t)g0 * P, ho.data(), sizeof(float) * ho.size(), cudaMemcpyHostToDevice));
+    if (r->any_iq_out) CU(cudaMemset(r->iqout.p + (size_t)g0 * r->nbmax * r->B, 0, sizeof(float2) * (size_t)C * r->nbmax * r->B));
+    Group& g = r->groups[d.group];
+    if (g.use_tc && (rc = rebuild_tc_tables(r, g)) != ABG_OK) return rc;  // the coefficient tables carry the bins
+    d.primed = false;
+    d.cur = 0;
+    d.fill = d.consumed = d.dropped = 0;
+    d.runs_since_compaction = 1;
+    d.ready.clear();
+    d.batch_seq = d.audio_seq = 0;
+    // the writes above use the legacy stream, which the engine's non-blocking streams are not ordered after
+    CU(cudaStreamSynchronize(0));
+    return ABG_OK;
+}
+
+int abg_follow_open(abg_engine* e, int dev, uint64_t first_batch, int n_channels, const abg_channel_cfg* channels, int queue_batches,
+                    int32_t* session) {
+    const HiDev* h = monitor_dev(e, e->history, dev, __func__);
+    if (!h) return ABG_ERANGE;
+    if (n_channels < 1 || !channels || queue_batches < 1 || !session)
+        return fail(ABG_EINVAL, "abg_follow_open: %d channels (%p), a queue of %d batches, session %p", n_channels, (const void*)channels,
+                    queue_batches, (void*)session);
+    if (!h->on()) return fail(ABG_ERANGE, "abg_follow_open: device %d has no history", dev);
+    const Device& d = e->dev[dev];
+    const unsigned __int128 S = (unsigned __int128)first_batch * e->B * d.hop;
+    if (S < h->first || S >= ((unsigned __int128)1 << 63))
+        return fail(ABG_ERANGE, "abg_follow_open: a session from batch %llu reads samples from %llu on; device %d's history holds [%llu, %llu)",
+                    (unsigned long long)first_batch, (unsigned long long)S, dev, (unsigned long long)h->first, (unsigned long long)h->end);
+    abg_engine::ReplayDevice want;
+    int rc = channel_shape(e, d, n_channels, channels, "abg_follow_open", &want);
+    if (rc != ABG_OK) return rc;
+    cudaSetDevice(e->cuda_dev);
+    // a free device of the session's shape, or a new follow engine with as many devices of it as exist already
+    int fi = -1, p = -1, have = 0;
+    for (int k = 0; k < (int)e->follow.size(); k++)
+        for (int q = 0; q < (int)e->follow[k].pool.size(); q++) {
+            if (!e->follow[k].pool[q].same_shape(want)) continue;
+            have++;
+            if (fi < 0 && e->follow[k].owner[q] < 0) {
+                fi = k;
+                p = q;
+            }
+        }
+    if (fi >= 0) {
+        abg_engine::FollowEngine& f = e->follow[fi];
+        f.pool[p].chans = want.chans;
+        if ((rc = follow_reset(f, p)) != ABG_OK) return rc;
+    } else {
+        const int n = std::max(have, 1);
+        abg_engine::FollowEngine f;
+        f.pool.assign(n, want);
+        f.owner.assign(n, -1);
+        std::vector<abg_device_cfg> devs(n, abg_device_cfg{want.sfmt, want.fullscale, want.sample_rate, n_channels, channels});
+        const abg_config cfg{e->N, e->W, e->fm_demod, n, devs.data()};
+        abg_options o{};
+        o.cuda_device = e->cuda_dev;
+        o.max_batches_per_run = e->nbmax;
+        o.fft_mode = e->fft_mode;
+        if ((rc = create_engine(&cfg, &o, true, &f.r)) != ABG_OK) return rc;
+        cudaSetDevice(e->cuda_dev);
+        if (cudaEventCreateWithFlags(&f.ev_compact, cudaEventDisableTiming) != cudaSuccess) {
+            engine_free(f.r);
+            return fail(ABG_ECUDA, "abg_follow_open: event creation failed");
+        }
+        e->follow.push_back(f);
+        fi = (int)e->follow.size() - 1;
+        p = 0;
+    }
+    const int32_t id = e->next_session++;
+    e->follow[fi].owner[p] = id;
+    abg_engine::FollowSession& s = e->sessions[id];
+    s.dev = dev;
+    s.eng = fi;
+    s.slot = p;
+    s.C = n_channels;
+    s.queue_batches = queue_batches;
+    s.first_batch = s.next_batch = first_batch;
+    *session = id;
+    return ABG_OK;
+}
+
+int abg_follow_close(abg_engine* e, int32_t session) {
+    abg_engine::FollowSession* s = follow_session(e, session, __func__);
+    if (!s) return ABG_ERANGE;
+    abg_engine::FollowEngine& f = e->follow[s->eng];
+    Device& d = f.r->dev[s->slot];
+    for (const auto& x : d.ready) f.r->slots[x.first].pending--;  // its unfetched batches give their result slots back
+    d.ready.clear();
+    f.owner[s->slot] = -1;
+    e->sessions.erase(session);
+    return ABG_OK;
+}
+
+// Move session s's finished batches out of its follow engine's result slots into its queue, oldest first, until the queue
+// holds `until` batches; with only_slot >= 0 only those in that slot.  Waits for the runs that computed them.
+static int follow_drain(abg_engine* e, abg_engine::FollowSession& s, int only_slot, size_t until) {
+    abg_engine* r = e->follow[s.eng].r;
+    Device& d = r->dev[s.slot];
+    const size_t B = r->B, C = s.C;
+    while (!d.ready.empty() && s.q.size() < until && (only_slot < 0 || d.ready.front().first == only_slot)) {
+        abg_engine::FollowBatch b;
+        b.wout.resize(C * B);
+        b.iq.resize(C * 2 * B);
+        b.axc.resize(C);
+        const int rc = abg_fetch_batch(r, s.slot, b.wout.data(), b.iq.data(), b.axc.data());
+        if (rc < 0) return rc;
+        s.q.push_back(std::move(b));
+    }
+    return ABG_OK;
+}
+
+// A (start, end) pair of timing events for the current abg_follow_run: kind 0 = a gather, 1 = a follow-engine run.
+static int follow_pair(abg_engine* e, int kind, int* idx) {
+    if (e->follow_tev.size() < 2 * (size_t)(e->follow_pairs + 1)) {
+        cudaEvent_t ev[2];
+        CU(cudaEventCreate(&ev[0]));
+        if (cudaEventCreate(&ev[1]) != cudaSuccess) {
+            cudaEventDestroy(ev[0]);
+            return fail(ABG_ECUDA, "abg_follow_run: event creation failed");
+        }
+        e->follow_tev.insert(e->follow_tev.end(), ev, ev + 2);
+        e->follow_kind.push_back(0);
+    }
+    e->follow_kind[e->follow_pairs] = kind;
+    *idx = 2 * e->follow_pairs++;
+    return ABG_OK;
+}
+
+int abg_follow_run(abg_engine* e, int max_batches) {
+    cudaSetDevice(e->cuda_dev);
+    e->follow_pairs = 0;
+    if (max_batches == 0 || e->sessions.empty()) return 0;
+    const long long budget = max_batches < 0 ? LLONG_MAX : max_batches;
+    const int B = e->B, N = e->N;
+    std::map<int32_t, long long> advanced;  // batches this call enqueued per session
+    int total = 0, rc;
+    for (;;) {
+        // the chunk: every session's next batches, as far as the history, its queue room, max_batches_per_run (one batch
+        // with AFC) and this call's max_batches allow, decided on the host from the enqueued history range
+        std::vector<std::vector<int>> nb(e->follow.size());
+        for (size_t k = 0; k < e->follow.size(); k++) nb[k].assign(e->follow[k].r->dev.size(), 0);
+        std::vector<bool> compacted(e->follow.size(), false);
+        std::vector<RpGather> g;
+        unsigned long long max_bytes = 0;
+        int chunk = 0;
+        for (auto& it : e->sessions) {
+            abg_engine::FollowSession& s = it.second;
+            if (s.lost) continue;
+            const Device& d = e->dev[s.dev];
+            const HiDev& h = e->history.dev[s.dev];
+            if (h.first == h.end) continue;
+            const unsigned long long S = s.first_batch * B * d.hop;
+            if (h.first > S + s.valid / d.bpc) {  // the history overwrote the next sample the session has not gathered
+                s.lost = true;
+                continue;
+            }
+            // batch b is available once (AGC_EXTRA + (b+1)*B)*hop + fft_size - hop <= end: for b < b_end
+            const unsigned long long fl = h.end + d.hop >= (unsigned long long)N ? (h.end + d.hop - N) / d.hop : 0;
+            const unsigned long long b_end = fl >= (unsigned long long)ABG_AGC_EXTRA ? (fl - ABG_AGC_EXTRA) / B : 0;
+            abg_engine::FollowEngine& f = e->follow[s.eng];
+            Device& rd = f.r->dev[s.slot];
+            const long long room = (long long)s.queue_batches - (long long)(s.q.size() + rd.ready.size());
+            const long long n = std::min({b_end > s.next_batch ? (long long)(b_end - s.next_batch) : 0ll, room,
+                                          (long long)(rd.has_afc ? 1 : f.r->nbmax), budget - advanced[it.first]});
+            if (n <= 0) continue;
+            // the bytes the fill rule needs for every batch so far (rtl_airband.cpp:394-400).  Its last hop samples may lie
+            // past the history's end; they are never read by these batches, and the next chunk gathers them again.
+            const unsigned long long done = s.next_batch - s.first_batch;
+            const unsigned long long want = ((ABG_AGC_EXTRA + (done + n) * B) * d.hop + N) * d.bpc;
+            const unsigned long long valid = std::min(want, (h.end - S) * d.bpc);
+            const size_t dropped = rd.dropped;
+            if ((rc = ingest_room(f.r, s.slot, want - s.pushed, "abg_follow_run")) != ABG_OK) return rc;
+            if (rd.dropped != dropped) compacted[s.eng] = true;
+            g.push_back(RpGather{h.ring.p, h.ring.n, S * d.bpc + s.valid, rd.raw[rd.cur] + rd.fill - (s.pushed - s.valid), want - s.valid});
+            max_bytes = std::max(max_bytes, want - s.valid);
+            rd.fill += want - s.pushed;
+            s.pushed = want;
+            s.valid = valid;
+            s.next_batch += n;
+            advanced[it.first] += n;
+            nb[s.eng][s.slot] = (int)n;
+            chunk += (int)n;
+        }
+        if (chunk == 0) break;
+        // the gather on the parent's K1 stream: behind every append it reads, ahead of every later one that would overwrite
+        // them.  Behind the chunk's compactions too: each waited for the follow engine's K1 that last read the buffer the
+        // gather now writes, and moved the bytes the previous chunk left past the history's end, which the gather replaces.
+        for (size_t k = 0; k < e->follow.size(); k++)
+            if (compacted[k]) {
+                CU(cudaEventRecord(e->follow[k].ev_compact, e->follow[k].r->stream_c));
+                CU(cudaStreamWaitEvent(e->stream, e->follow[k].ev_compact, 0));
+            }
+        // upload_small writes whole 16-byte words: one record of room for the rounding
+        if (e->follow_gather.n < g.size() + 1) {
+            e->follow_gather.free();
+            if (e->follow_gather.alloc(2 * g.size() + 1)) return fail(ABG_ENOMEM, "Out of device memory for the live follow");
+        }
+        const int nl = upload_small(e->follow_gather.p, g.data(), sizeof(RpGather) * g.size(), e->stream);
+        if (nl < 0) return fail(ABG_ECUDA, "live follow parameter upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+        e->launches += (uint64_t)nl;
+        int ig;
+        if ((rc = follow_pair(e, 0, &ig)) != ABG_OK) return rc;
+        CU(cudaEventRecord(e->follow_tev[ig], e->stream));
+        const cudaError_t er = abg_launch_replay_gather(e->follow_gather.p, (int)g.size(), abg_history_blocks(max_bytes, (int)g.size(), e->sm_count), e->stream);
+        if (er != cudaSuccess) return fail(ABG_ECUDA, "live follow gather launch failed: %s", cudaGetErrorString(er));
+        e->launches++;
+        const cudaEvent_t gathered = e->follow_tev[ig + 1];
+        CU(cudaEventRecord(gathered, e->stream));
+        // one run per follow engine with work; its ingest stream, and so its K1 and later compactions, wait for the gather
+        for (size_t k = 0; k < e->follow.size(); k++) {
+            if (std::all_of(nb[k].begin(), nb[k].end(), [](int v) { return v == 0; })) continue;
+            abg_engine::FollowEngine& f = e->follow[k];
+            abg_engine* r = f.r;
+            CU(cudaStreamWaitEvent(r->stream_c, gathered, 0));
+            r->ingest_dirty = true;
+            // the result slot this run exports into: move what it still holds into the sessions' queues
+            const int sl = r->next_slot;
+            for (size_t q = 0; q < f.owner.size() && r->slots[sl].pending > 0; q++)
+                if (f.owner[q] >= 0 && (rc = follow_drain(e, e->sessions[f.owner[q]], sl, SIZE_MAX)) != ABG_OK) return rc;
+            int it;
+            if ((rc = follow_pair(e, 1, &it)) != ABG_OK) return rc;
+            CU(cudaStreamWaitEvent(r->stream, gathered, 0));
+            CU(cudaEventRecord(e->follow_tev[it], r->stream));
+            int ran = 0;
+            if ((rc = enqueue_run(r, nb[k], false, true, &ran)) != ABG_OK) return rc;
+            CU(cudaEventRecord(e->follow_tev[it + 1], r->stream_b));
+        }
+        total += chunk;
+    }
+    return total;
+}
+
+int abg_follow_fetch(abg_engine* e, int32_t session, int max_batches, float* waveout, float* iq_out, char* axcindicate,
+                     uint64_t* first_batch) {
+    abg_engine::FollowSession* s = follow_session(e, session, __func__);
+    if (!s) return ABG_ERANGE;
+    if (max_batches < 0 || (max_batches > 0 && (!waveout || !axcindicate)))
+        return fail(ABG_EINVAL, "abg_follow_fetch: %d batches into waveout %p, axcindicate %p", max_batches, (void*)waveout, (void*)axcindicate);
+    const Device& rd = e->follow[s->eng].r->dev[s->slot];
+    const uint64_t first = s->next_batch - (uint64_t)(s->q.size() + rd.ready.size());  // the oldest unfetched batch
+    cudaSetDevice(e->cuda_dev);
+    const int rc = follow_drain(e, *s, -1, (size_t)max_batches);
+    if (rc != ABG_OK) return rc;
+    if (s->q.empty() && s->lost)
+        return fail(ABG_ERANGE, "abg_follow_fetch: session %d is lost: device %d's history overwrote batch %llu before it was read", (int)session,
+                    s->dev, (unsigned long long)s->next_batch);
+    const int n = (int)std::min<size_t>((size_t)max_batches, s->q.size());
+    const size_t C = s->C, B = e->B;
+    for (int k = 0; k < n; k++) {
+        const abg_engine::FollowBatch& b = s->q.front();
+        memcpy(waveout + k * C * B, b.wout.data(), sizeof(float) * C * B);
+        if (iq_out) memcpy(iq_out + k * C * 2 * B, b.iq.data(), sizeof(float) * C * 2 * B);
+        memcpy(axcindicate + k * C, b.axc.data(), C);
+        s->q.pop_front();
+    }
+    if (first_batch) *first_batch = first;
+    return n;
+}
+
+int abg_follow_info(abg_engine* e, int32_t session, abg_follow_status* out) {
+    const abg_engine::FollowSession* s = follow_session(e, session, __func__);
+    if (!s) return ABG_ERANGE;
+    if (!out) return fail(ABG_EINVAL, "abg_follow_info: null argument");
+    out->dev = s->dev;
+    out->n_channels = s->C;
+    out->next_batch = s->next_batch;
+    out->queued = (int32_t)(s->q.size() + e->follow[s->eng].r->dev[s->slot].ready.size());
+    out->lost = s->lost ? 1 : 0;
+    return ABG_OK;
+}
+
+int abg_follow_stats(abg_engine* e, int32_t session, int chan, abg_squelch_stats* out) {
+    const abg_engine::FollowSession* s = follow_session(e, session, __func__);
+    if (!s) return ABG_ERANGE;
+    if (chan < 0 || chan >= s->C) return fail(ABG_ERANGE, "abg_follow_stats: channel %d out of range", chan);
+    if (!out) return fail(ABG_EINVAL, "abg_follow_stats: null argument");
+    return abg_get_stats(e->follow[s->eng].r, s->slot, chan, out);
+}
+
+int abg_debug_follow_time(abg_engine* e, float* ms2) {
+    if (!ms2) return fail(ABG_EINVAL, "abg_debug_follow_time: null argument");
+    ms2[0] = ms2[1] = 0.0f;
+    cudaSetDevice(e->cuda_dev);
+    for (int k = 0; k < e->follow_pairs; k++) {
+        float ms = 0.0f;
+        CU(cudaEventSynchronize(e->follow_tev[2 * k + 1]));
+        CU(cudaEventElapsedTime(&ms, e->follow_tev[2 * k], e->follow_tev[2 * k + 1]));
+        ms2[e->follow_kind[k]] += ms;
+    }
     return ABG_OK;
 }
 

@@ -31,6 +31,8 @@ SYMBOLS = [
     "abg_activity_configure", "abg_fetch_activity", "abg_debug_activity_time",
     "abg_history_configure", "abg_history_range", "abg_history_raw", "abg_history_subband", "abg_debug_history_time",
     "abg_history_replay", "abg_debug_replay_time",
+    "abg_follow_open", "abg_follow_close", "abg_follow_run", "abg_follow_fetch", "abg_follow_info", "abg_follow_stats",
+    "abg_debug_follow_time",
 ]
 
 SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
@@ -98,6 +100,17 @@ class CReplayJob(C.Structure):
         ("iq_out", C.c_void_p),
         ("axcindicate", C.c_void_p),
         ("stats", C.POINTER(CSquelchStats)),
+    ]
+
+
+class CFollowStatus(C.Structure):
+    """abg_follow_status: what abg_follow_info reports of a live follow session (definition in airband_b200.h)."""
+    _fields_ = [
+        ("dev", C.c_int32),
+        ("n_channels", C.c_int32),
+        ("next_batch", C.c_uint64),
+        ("queued", C.c_int32),
+        ("lost", C.c_int32),
     ]
 
 
@@ -196,6 +209,15 @@ def load():
     L.abg_debug_history_time.restype, L.abg_debug_history_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_history_replay.restype, L.abg_history_replay.argtypes = i, [vp, i, C.POINTER(CReplayJob)]
     L.abg_debug_replay_time.restype, L.abg_debug_replay_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_follow_open.restype = i
+    L.abg_follow_open.argtypes = [vp, i, C.c_uint64, i, C.POINTER(CChannelCfg), i, C.POINTER(C.c_int32)]
+    L.abg_follow_close.restype, L.abg_follow_close.argtypes = i, [vp, C.c_int32]
+    L.abg_follow_run.restype, L.abg_follow_run.argtypes = i, [vp, i]
+    L.abg_follow_fetch.restype = i
+    L.abg_follow_fetch.argtypes = [vp, C.c_int32, i, vp, vp, vp, C.POINTER(C.c_uint64)]
+    L.abg_follow_info.restype, L.abg_follow_info.argtypes = i, [vp, C.c_int32, C.POINTER(CFollowStatus)]
+    L.abg_follow_stats.restype, L.abg_follow_stats.argtypes = i, [vp, C.c_int32, i, C.POINTER(CSquelchStats)]
+    L.abg_debug_follow_time.restype, L.abg_debug_follow_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -587,6 +609,57 @@ class Engine:
         """(gather ms, replay engine run ms) of the most recent history_replay, from CUDA events; 0 before the first."""
         ms = (C.c_float * 2)()
         self._chk(self.L.abg_debug_replay_time(self.h, ms))
+        return float(ms[0]), float(ms[1])
+
+    # ---- live follow ----------------------------------------------------------------------------------------------
+    def follow_open(self, dev: int, first_batch: int, channels, queue_batches: int = 16) -> int:
+        """Open a live follow session (definition in airband_b200.h): a history replay of device dev from first_batch on,
+        with no end, that follow_run keeps advancing as the history grows.  channels: a list of config.Channel, e.g.
+        from transmission_follow (follow_open(**job)).  Returns the session id."""
+        chans = channels_to_c(channels)
+        sid = C.c_int32(-1)
+        self._chk(self.L.abg_follow_open(self.h, int(dev), int(first_batch), len(channels), C.cast(chans, C.POINTER(CChannelCfg)),
+                                         int(queue_batches), C.byref(sid)))
+        return int(sid.value)
+
+    def follow_close(self, session: int) -> None:
+        self._chk(self.L.abg_follow_close(self.h, int(session)))
+
+    def follow_run(self, max_batches: int = -1) -> int:
+        """Advance every open session by up to max_batches batches (< 0: as far as the history and queue room allow);
+        returns the session-batches enqueued.  Does not wait for the live engine."""
+        return self._chk(self.L.abg_follow_run(self.h, int(max_batches)))
+
+    def follow_info(self, session: int) -> dict:
+        """dev, n_channels, next_batch (the next batch follow_run enqueues), queued (unfetched batches) and lost."""
+        st = CFollowStatus()
+        self._chk(self.L.abg_follow_info(self.h, int(session), C.byref(st)))
+        return dict(dev=st.dev, n_channels=st.n_channels, next_batch=int(st.next_batch), queued=st.queued, lost=bool(st.lost))
+
+    def follow_fetch(self, session: int, max_batches: Optional[int] = None, want_iq: bool = True) -> dict:
+        """Pop up to max_batches (default: every queued one) of a session's oldest batches, waiting for them: a dict with
+        first_batch (batch number of the first, None if none was popped), waveout float32[n, C, B], iq complex64[n, C, B]
+        (None unless want_iq) and axc uint8[n, C].  Raises AbgError (ABG_ERANGE) once a lost session has nothing left."""
+        info = self.follow_info(session)
+        n, Cn = info["queued"] if max_batches is None else int(max_batches), info["n_channels"]
+        wo = np.zeros((max(n, 0), Cn, self.B), np.float32)
+        iq = np.zeros((max(n, 0), Cn, 2 * self.B), np.float32) if want_iq else None
+        ax = np.zeros((max(n, 0), Cn), np.uint8)
+        first = C.c_uint64(0)
+        got = self._chk(self.L.abg_follow_fetch(self.h, int(session), n, _ptr(wo), _ptr(iq), _ptr(ax), C.byref(first)))
+        return dict(first_batch=int(first.value) if got else None, waveout=wo[:got],
+                    iq=iq[:got].view(np.complex64) if want_iq else None, axc=ax[:got])
+
+    def follow_stats(self, session: int, chan: int) -> CSquelchStats:
+        """Squelch statistics of a session's channel after its batch next_batch - 1 (waits for it)."""
+        st = CSquelchStats()
+        self._chk(self.L.abg_follow_stats(self.h, int(session), int(chan), C.byref(st)))
+        return st
+
+    def follow_time(self) -> Tuple[float, float]:
+        """(gather ms, follow-engine run ms) of the most recent follow_run, from CUDA events; 0 if it enqueued nothing."""
+        ms = (C.c_float * 2)()
+        self._chk(self.L.abg_debug_follow_time(self.h, ms))
         return float(ms[0]), float(ms[1])
 
     # ---- mixers ---------------------------------------------------------------------------------------------------
@@ -984,6 +1057,21 @@ def transmission_capture(tx: dict, cfg: Config, dev: int, history_range: Tuple[i
 REPLAY_SETTLE_BATCHES = 6
 
 
+def _lead_in_batch(tx: dict, cfg: Config, dev: int, history_range: Tuple[int, int], lead_s: Optional[float], fn: str):
+    """(first batch, lead_s) of a replay or follow session for one transmission: the latest batch whose first frame lies
+    at least lead_s seconds of frames (default REPLAY_SETTLE_BATCHES batches) before the transmission's first frame, or
+    the first batch whose samples the history holds if that is later."""
+    B, hop = cfg.wave_batch, cfg.hop(dev)
+    if lead_s is None:
+        lead_s = REPLAY_SETTLE_BATCHES * B / cfg.wave_rate
+    if lead_s < 0:
+        raise ValueError(f"{fn}: lead_s must be >= 0")
+    lead = int(np.ceil(lead_s * cfg.devices[dev].sample_rate / hop))  # frames
+    b_lead = (int(tx["first_frame"]) - AGC_EXTRA - lead) // B
+    b_first = -(-int(history_range[0]) // (B * hop))
+    return max(b_lead, b_first, 0), lead_s
+
+
 def transmission_replay(tx: dict, cfg: Config, dev: int, history_range: Tuple[int, int], lead_s: Optional[float] = None,
                         **channel_kw) -> dict:
     """An Engine.history_replay job that listens to one transmission (a group_transmissions dict of device dev): a channel
@@ -997,15 +1085,8 @@ def transmission_replay(tx: dict, cfg: Config, dev: int, history_range: Tuple[in
     nothing of the transmission fits."""
     d = cfg.devices[dev]
     B, hop, N = cfg.wave_batch, cfg.hop(dev), cfg.fft_size
-    if lead_s is None:
-        lead_s = REPLAY_SETTLE_BATCHES * B / cfg.wave_rate
-    if lead_s < 0:
-        raise ValueError("transmission_replay: lead_s must be >= 0")
+    b0, lead_s = _lead_in_batch(tx, cfg, dev, history_range, lead_s, "transmission_replay")
     first, end = history_range
-    lead = int(np.ceil(lead_s * d.sample_rate / hop))  # frames
-    b_lead = (int(tx["first_frame"]) - AGC_EXTRA - lead) // B
-    b_first = -(-int(first) // (B * hop))
-    b0 = max(b_lead, b_first, 0)
     b_last = (int(tx["last_frame"]) - AGC_EXTRA) // B
     b_end = ((int(end) - N + hop) // hop - AGC_EXTRA) // B  # batches b < b_end have every sample in the history
     n = min(b_last + 1, b_end) - b0
@@ -1014,3 +1095,15 @@ def transmission_replay(tx: dict, cfg: Config, dev: int, history_range: Tuple[in
                          f"the history [{first}, {end}) with {lead_s} s of lead-in")
     ch = make_channel(int(round(tx["freq_hz"])), d.centerfreq, d.sample_rate, N, cfg.wave_rate, **channel_kw)
     return dict(dev=dev, first_batch=b0, n_batches=n, channels=[ch])
+
+
+def transmission_follow(tx: dict, cfg: Config, dev: int, history_range: Tuple[int, int], lead_s: Optional[float] = None,
+                        **channel_kw) -> dict:
+    """An Engine.follow_open session that listens to one transmission (a group_transmissions dict of device dev) from its
+    lead-in on and keeps listening as the history grows: dev, first_batch and channels as transmission_replay gives
+    them (same channel, same start rule), with no end.  first_batch may lie past the history's end when the
+    transmission was reported ahead of it; the session then waits for its samples."""
+    d = cfg.devices[dev]
+    b0, _ = _lead_in_batch(tx, cfg, dev, history_range, lead_s, "transmission_follow")
+    ch = make_channel(int(round(tx["freq_hz"])), d.centerfreq, d.sample_rate, cfg.fft_size, cfg.wave_rate, **channel_kw)
+    return dict(dev=dev, first_batch=b0, channels=[ch])
