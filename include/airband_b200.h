@@ -618,6 +618,67 @@ ABG_API int abg_follow_stats(abg_engine* e, int32_t session, int chan, abg_squel
  * (from the end of the chunk's gather to the end of the run, summed); 0 if it enqueued nothing.  Waits for them. */
 ABG_API int abg_debug_follow_time(abg_engine* e, float* ms2);
 
+/* History analysis (not part of the reference surface: the band spectrum and the activity detector only see the batches
+ * after they are switched on, with the settings they had then, so "what was on the band 20 s ago" has no answer unless
+ * they were on and set right).  Both can be run over any window of a device's I/Q history, with any settings, after the
+ * fact.  Names as for the history: frame f reads the samples [f*hop, f*hop + fft_size), and batch b covers the frames
+ * AGC_EXTRA + b*B + j, j in [0, B), B = WAVE_BATCH.
+ *   Spectrogram: a job names dev, first_frame, n_rows >= 1, frames_per_row F >= 1 and a stride 1 <= s <= F.  Row r covers
+ *     the frames first_frame + r*F + j, j in [0, F); those with j % s == 0 are selected, n = ceil(F / s) of them, and the row
+ *     is the band spectrum's P[k] = (1/n) * sum |X_f[k]|^2 over them: the same conversion, window, FFT and float32
+ *     expression, summed in the same order (chunks of 32 selected frames, each in frame order, then the chunk sums in chunk
+ *     order).  So with F = B and first_frame = AGC_EXTRA + b*B, row r is bitwise the live spectrum of batch b + r at stride s;
+ *     any other F (or a first_frame off the batch grid) is the same arithmetic on other frames.
+ *   Activity: a job names dev, first_batch, n_batches >= 1 and the detector's stride, hang, min_span and thr[fft_size],
+ *     checked as abg_activity_configure checks them.  Its result is the merged bursts over the window: the pieces the live
+ *     detector emits for those batches with those settings, joined as merging joins them, except at the window's edges.  A
+ *     burst whose first piece had OPEN_START in the window's first batch carries ABG_BURST_OPEN_START, one whose last piece
+ *     had OPEN_END in the last batch carries ABG_BURST_OPEN_END, and such edge bursts are kept even with a span below
+ *     min_span, since they may continue outside the window; every other burst has flags 0.  Bursts are sorted by (bin,
+ *     first_frame), a joined burst's sum is the float32 sum of its pieces' sums in batch order, and every field is bitwise
+ *     reproducible.  A batch with more than ABG_ACTIVITY_MAX_RECORDS pieces is counted in n_truncated; the bursts of such a
+ *     batch are unspecified, as in a truncated live reading.
+ *   Window: every sample of every selected frame must lie in abg_history_range (ABG_ERANGE otherwise, the message gives the
+ *     range needed).  A batch's last frames reach fft_size - hop samples into the next batch, so the newest history batch
+ *     can be analysed once its successor has been appended, the same lag as live follow.
+ * Results do not depend on how jobs are grouped into calls or ordered, on max_batches_per_run or the push pattern, on
+ * whether the live spectrum or detector is on, or on other calls in between.  Several jobs may name the same device.  A
+ * scan-mode retune inside a window mixes both tunings, as for a capture.
+ * Computed on the GPU by the band spectrum's and the detector's own kernels: per chunk, one gather launch on the K1 stream
+ * copies every job's window from its history ring into a private scratch buffer (behind every append it reads, ahead of
+ * every later one that would overwrite them), then one spectrum or detector launch covers every job.  Partial sums,
+ * counters, thresholds, scratch and results are the calls' own: the live monitors are untouched and live runs launch
+ * nothing new.  Nothing is allocated before the first call; everything is freed when the last history is switched off and
+ * by abg_destroy.  The calls wait for their results.  ABG_EINVAL for n_jobs outside [1, 65535] or a null jobs. */
+typedef struct abg_spectrogram_job {
+    int32_t dev;
+    int32_t n_rows;          /* >= 1 */
+    uint64_t first_frame;    /* absolute frame number of row 0's first frame */
+    int32_t frames_per_row;  /* F >= 1 */
+    int32_t stride;          /* 1 <= stride <= F */
+    float* power;            /* [n_rows][fft_size], caller memory */
+} abg_spectrogram_job;
+/* ABG_ERANGE for a bad dev or a window outside the history (also when the history is off); ABG_EINVAL for n_rows < 1, F < 1,
+ * a stride outside [1, F] and a null power. */
+ABG_API int abg_history_spectrogram(abg_engine* e, int n_jobs, const abg_spectrogram_job* jobs);
+typedef struct abg_activity_job {
+    int32_t dev;
+    int32_t n_batches;       /* >= 1 */
+    uint64_t first_batch;
+    int32_t stride, hang, min_span;
+    int32_t cap;             /* room in out, >= 0 */
+    const float* thr;        /* [fft_size] */
+    abg_burst* out;          /* [cap], caller memory; may be NULL with cap = 0 */
+    int32_t n_bursts;        /* written: bursts found; the first min(n_bursts, cap) of them are stored */
+    int32_t n_truncated;     /* written: batches with more than ABG_ACTIVITY_MAX_RECORDS pieces */
+} abg_activity_job;
+/* ABG_ERANGE for a bad dev or a window outside the history (also when the history is off); ABG_EINVAL for what
+ * abg_activity_configure refuses with stride > 0, for stride 0, n_batches < 1, cap < 0 and a null out with cap > 0. */
+ABG_API int abg_history_activity(abg_engine* e, int n_jobs, abg_activity_job* jobs);
+/* Measurement aid: device time of the most recent abg_history_spectrogram or abg_history_activity, summed over its chunks:
+ * ms3[0] = its gathers, ms3[1] = its spectrum kernels, ms3[2] = its detector kernels; 0 where it had none. */
+ABG_API int abg_debug_history_analysis_time(abg_engine* e, float* ms3);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

@@ -23,6 +23,7 @@
 #include <cstdint>
 #include <complex>
 #include <deque>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -591,6 +592,19 @@ struct abg_engine {
     std::vector<cudaEvent_t> follow_tev;  // (start, end) pairs: the latest abg_follow_run's gathers and runs
     std::vector<int> follow_kind;         // per pair: 0 = gather, 1 = follow-engine run
     int follow_pairs = 0;
+    // history analysis (abg_history_spectrogram, abg_history_activity): the calls' own buffers, never the live monitors';
+    // created by the first call, freed when the last history is switched off
+    struct Analysis {
+        DevBuf<unsigned char> scratch;   // one chunk's gathered window bytes
+        DevBuf<unsigned char> work;      // one chunk's spectrum chunk sums, then int32 counters per row (zero between launches)
+        DevBuf<unsigned char> table;     // one chunk's gather records, kernel tables and thresholds
+        unsigned char* h_table = nullptr;  // page-locked staging of `table`
+        size_t h_table_bytes = 0;
+        unsigned char* result = nullptr;   // page-locked, mapped: one chunk's spectrogram rows or detector entries
+        size_t result_bytes = 0;
+        cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // gather start, gather end, kernel end
+        float ms[3] = {0.0f, 0.0f, 0.0f};  // the latest call: gathers, spectrum kernels, detector kernels
+    } analysis;
 
     K2Launch k2_launch(int cur) const {
         K2Launch L{};
@@ -756,6 +770,22 @@ void follow_free(abg_engine* e) {
     e->follow_pairs = 0;
 }
 
+// The history analysis buffers and events (abg_history_spectrogram, abg_history_activity).
+void analysis_free(abg_engine* e) {
+    auto& a = e->analysis;
+    a.scratch.free();
+    a.work.free();
+    a.table.free();
+    if (a.h_table) cudaFreeHost(a.h_table);
+    if (a.result) cudaFreeHost(a.result);
+    a.h_table = a.result = nullptr;
+    a.h_table_bytes = a.result_bytes = 0;
+    for (auto& ev : a.ev) {
+        if (ev) cudaEventDestroy(ev);
+        ev = nullptr;
+    }
+}
+
 void engine_free(abg_engine* e) {
     if (!e) return;
     cudaSetDevice(e->cuda_dev);
@@ -763,6 +793,7 @@ void engine_free(abg_engine* e) {
     if (e->stream_b) cudaStreamSynchronize(e->stream_b);
     replay_free(e);
     follow_free(e);
+    analysis_free(e);
     for (auto& d : e->dev) {
         for (int i = 0; i < 2; i++)
             if (d.raw[i]) cudaFree(d.raw[i]);
@@ -2126,22 +2157,31 @@ int abg_fetch_tone_meter(abg_engine* e, int dev, float* tones, float* energy, in
 int abg_debug_tone_meter_time(abg_engine* e, float* ms) { return monitor_time(e, e->tone_meter, ms, __func__); }
 
 // ---- band activity detector (definition in airband_b200.h) ----------------------------------------------------------
+// The detector settings abg_activity_configure accepts, for abg_activity_configure and abg_history_activity (fn names the
+// caller in errors): stride 0 passes here and means off.
+static int activity_check(const abg_engine* e, const char* fn, int stride, int hang, int min_span, const float* thr) {
+    if (stride < 0 || hang < 0 || min_span < 0)
+        return fail(ABG_EINVAL, "%s: negative argument (stride %d, hang %d, min_span %d)", fn, stride, hang, min_span);
+    const int N = e->N, B = e->B;
+    if (stride > 0) {
+        if (stride > B) return fail(ABG_EINVAL, "%s: stride %d exceeds the batch of %d frames", fn, stride, B);
+        const int n_sel = (B + stride - 1) / stride;
+        if (hang >= n_sel) return fail(ABG_EINVAL, "%s: hang %d is not below the %d selected frames of a batch", fn, hang, n_sel);
+        if (min_span < 1) return fail(ABG_EINVAL, "%s: min_span %d is below 1", fn, min_span);
+        if (!thr) return fail(ABG_EINVAL, "%s: null thresholds", fn);
+        for (int k = 0; k < N; k++)
+            if (!std::isfinite(thr[k]) || !(thr[k] > 0.0f))
+                return fail(ABG_EINVAL, "%s: threshold of bin %d (%g) is not finite and positive", fn, k, (double)thr[k]);
+    }
+    return ABG_OK;
+}
+
 int abg_activity_configure(abg_engine* e, int dev, int stride, int hang, int min_span, const float* thr) {
     ActDev* d = monitor_dev(e, e->activity, dev, __func__);
     if (!d) return ABG_ERANGE;
-    if (stride < 0 || hang < 0 || min_span < 0)
-        return fail(ABG_EINVAL, "abg_activity_configure: negative argument (stride %d, hang %d, min_span %d)", stride, hang, min_span);
+    const int rc_check = activity_check(e, __func__, stride, hang, min_span, thr);
+    if (rc_check != ABG_OK) return rc_check;
     const int N = e->N, B = e->B;
-    if (stride > 0) {
-        if (stride > B) return fail(ABG_EINVAL, "abg_activity_configure: stride %d exceeds the batch of %d frames", stride, B);
-        const int n_sel = (B + stride - 1) / stride;
-        if (hang >= n_sel) return fail(ABG_EINVAL, "abg_activity_configure: hang %d is not below the %d selected frames of a batch", hang, n_sel);
-        if (min_span < 1) return fail(ABG_EINVAL, "abg_activity_configure: min_span %d is below 1", min_span);
-        if (!thr) return fail(ABG_EINVAL, "abg_activity_configure: null thresholds");
-        for (int k = 0; k < N; k++)
-            if (!std::isfinite(thr[k]) || !(thr[k] > 0.0f))
-                return fail(ABG_EINVAL, "abg_activity_configure: threshold of bin %d (%g) is not finite and positive", k, (double)thr[k]);
-    }
     if (stride == 0 && d->stride == 0) return ABG_OK;
     const int rc = monitor_configure(e, e->activity, stride > 0);  // an enqueued detector kernel may still read the thresholds
     if (rc != ABG_OK) return rc;
@@ -2228,9 +2268,10 @@ int abg_history_configure(abg_engine* e, int dev, int n_batches) {
         c.ring_bytes = s.ring.n;
         return ABG_OK;
     });
-    if (e->history.devs.empty()) {  // nothing left to replay or follow (no session is open: see above)
+    if (e->history.devs.empty()) {  // nothing left to replay, follow or analyse (no session is open: see above)
         replay_free(e);
         follow_free(e);
+        analysis_free(e);
     }
     return rc != ABG_OK ? rc : rp;
 }
@@ -2873,6 +2914,406 @@ int abg_debug_follow_time(abg_engine* e, float* ms2) {
         CU(cudaEventElapsedTime(&ms, e->follow_tev[2 * k], e->follow_tev[2 * k + 1]));
         ms2[e->follow_kind[k]] += ms;
     }
+    return ABG_OK;
+}
+
+// ---- history analysis (definition in airband_b200.h) ---------------------------------------------------------------------
+// A job is a run of units of one device, spectrogram rows or detector batches: unit u starts at frame base + u*step and
+// selects n_sel frames `stride` apart.  A call is cut into chunks of whole units within fixed budgets.  Per chunk, the
+// replay gather copies each job's share of the window from its history ring into the scratch buffer, at the stream byte's
+// offset modulo 16 (the alignment the live raw buffer gives it), and one launch of the live monitor's kernel reads it there.
+constexpr size_t kAnalysisScratch = 64ull << 20;  // gathered bytes per chunk: a 10 s window of one cfg2 device is 51 MB
+constexpr size_t kAnalysisWork = 64ull << 20;     // spectrum chunk sums per chunk
+constexpr size_t kAnalysisResult = 32ull << 20;   // page-locked results per chunk: rows of fft_size floats, detector entries of 160 KB
+constexpr int kAnalysisMaxUnits = 65535;          // rows of a spectrum launch (its grid.y), pieces of a detector launch
+
+struct AnJob {
+    int dev;
+    unsigned __int128 base;    // frames
+    unsigned long long step;   // frames
+    int n_units, n_sel, stride;
+    size_t unit_result, unit_work;  // bytes per unit
+};
+struct AnPiece {  // units [u0, u0 + n) of job `job`: stream bytes [src, src + bytes) at scratch offset off
+    int job, u0, n;
+    unsigned long long src, off, bytes;
+};
+
+static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+// The samples units [u0, u0 + n) of job J read: [*first, *end).  128 bits, so that a window far past the history is
+// refused rather than wrapped.
+static void analysis_span(const abg_engine* e, const AnJob& J, long long u0, long long n, unsigned __int128* first, unsigned __int128* end) {
+    const unsigned hop = (unsigned)e->dev[J.dev].hop;
+    const unsigned __int128 f0 = J.base + (unsigned __int128)u0 * J.step;
+    *first = f0 * hop;
+    *end = (f0 + (unsigned __int128)(n - 1) * J.step + (unsigned __int128)(J.n_sel - 1) * J.stride) * hop + (unsigned)e->N;
+}
+
+static int analysis_window(abg_engine* e, const char* fn, int j, const AnJob& J) {
+    const HiDev& h = e->history.dev[J.dev];
+    unsigned __int128 lo, hi;
+    analysis_span(e, J, 0, J.n_units, &lo, &hi);
+    if (h.first == h.end || lo < h.first || hi > h.end)
+        return fail(ABG_ERANGE, "%s: job %d reads samples [%llu, %llu) of device %d, outside its history [%llu, %llu)", fn, j,
+                    (unsigned long long)lo, (unsigned long long)hi, J.dev, (unsigned long long)h.first, (unsigned long long)h.end);
+    return ABG_OK;
+}
+
+// Buffers for chunks of the jobs' units (they only grow, each to its budget or to the largest single unit), the events,
+// and the times reset.
+static int analysis_prepare(abg_engine* e, const std::vector<AnJob>& jobs, size_t* scratch_cap, size_t* work_cap, size_t* result_cap) {
+    auto& a = e->analysis;
+    size_t sc = kAnalysisScratch, wk = kAnalysisWork, rs = kAnalysisResult;
+    for (const AnJob& J : jobs) {
+        unsigned __int128 lo, hi;
+        analysis_span(e, J, 0, 1, &lo, &hi);
+        sc = std::max(sc, (size_t)(hi - lo) * e->dev[J.dev].bpc + 32);
+        wk = std::max(wk, J.unit_work);
+        rs = std::max(rs, J.unit_result);
+    }
+    cudaSetDevice(e->cuda_dev);
+    if (!a.ev[0])
+        for (auto& ev : a.ev) CU(cudaEventCreate(&ev));
+    if (a.scratch.n < sc) {
+        a.scratch.free();
+        if (a.scratch.alloc(sc)) return fail(ABG_ENOMEM, "Out of device memory for the history analysis scratch (%zu bytes)", sc);
+    }
+    const size_t counters = sizeof(int32_t) * kAnalysisMaxUnits;
+    if (a.work.n < wk + counters) {
+        a.work.free();
+        if (a.work.alloc(wk + counters)) return fail(ABG_ENOMEM, "Out of device memory for the history analysis sums (%zu bytes)", wk);
+        CU(cudaMemsetAsync(a.work.p + wk, 0, counters, e->stream));
+    }
+    if (a.result_bytes < rs) {
+        if (a.result) cudaFreeHost(a.result);
+        a.result = nullptr;
+        a.result_bytes = 0;
+        if (cudaHostAlloc((void**)&a.result, rs, cudaHostAllocMapped) != cudaSuccess) {
+            cudaGetLastError();
+            a.result = nullptr;
+            return fail(ABG_ENOMEM, "Out of page-locked host memory for the history analysis results (%zu bytes)", rs);
+        }
+        a.result_bytes = rs;
+    }
+    *scratch_cap = a.scratch.n;
+    *work_cap = a.work.n - counters;
+    *result_cap = a.result_bytes;
+    a.ms[0] = a.ms[1] = a.ms[2] = 0.0f;
+    return ABG_OK;
+}
+
+// Cut the jobs' units into chunks, in job and unit order, and call run(pieces) for each: a chunk's gathered bytes, results
+// and spectrum sums stay within the buffers, its units and pieces within kAnalysisMaxUnits.
+static int analysis_chunks(abg_engine* e, const std::vector<AnJob>& jobs, const std::function<int(const std::vector<AnPiece>&)>& run) {
+    size_t scratch_cap, work_cap, result_cap;
+    int rc = analysis_prepare(e, jobs, &scratch_cap, &work_cap, &result_cap);
+    if (rc != ABG_OK) return rc;
+    std::vector<AnPiece> ps;
+    size_t used_res = 0, used_work = 0;
+    int units = 0;
+    for (int j = 0; j < (int)jobs.size(); j++) {
+        const AnJob& J = jobs[j];
+        const int bpc = e->dev[J.dev].bpc;
+        for (int u = 0; u < J.n_units; u++) {
+            for (;;) {
+                const bool extend = !ps.empty() && ps.back().job == j;
+                AnPiece p = extend ? ps.back() : AnPiece{j, u, 0, 0, 0, 0};
+                unsigned __int128 lo, hi;
+                analysis_span(e, J, p.u0, p.n + 1, &lo, &hi);
+                p.n++;
+                p.src = (unsigned long long)lo * bpc;
+                p.bytes = (unsigned long long)(hi - lo) * bpc;
+                if (!extend) p.off = align16(ps.empty() ? 0 : ps.back().off + ps.back().bytes) + p.src % 16;
+                const bool fits = p.off + p.bytes <= scratch_cap && used_res + J.unit_result <= result_cap &&
+                                  used_work + J.unit_work <= work_cap && units < kAnalysisMaxUnits;
+                if (fits || ps.empty()) {  // (a unit alone always fits: the buffers were sized for it)
+                    if (extend)
+                        ps.back() = p;
+                    else
+                        ps.push_back(p);
+                    used_res += J.unit_result;
+                    used_work += J.unit_work;
+                    units++;
+                    break;
+                }
+                if ((rc = run(ps)) != ABG_OK) return rc;
+                ps.clear();
+                used_res = used_work = 0;
+                units = 0;
+            }
+        }
+    }
+    return ps.empty() ? ABG_OK : run(ps);
+}
+
+// One chunk on the K1 stream: the upload of its records, the gather of every piece into the scratch (behind every append
+// it reads, ahead of every later one that would overwrite its bytes), then kernel(device tables, stream).  fill(host
+// tables) writes `tables` bytes of kernel records first.  Waits for the chunk and adds the gather's device time to ms[0],
+// the kernel's to ms[which].
+static int analysis_launch(abg_engine* e, const std::vector<AnJob>& jobs, const std::vector<AnPiece>& ps, size_t tables, int which,
+                           const std::function<void(unsigned char*)>& fill,
+                           const std::function<cudaError_t(unsigned char*, cudaStream_t)>& kernel) {
+    auto& a = e->analysis;
+    const size_t gb = align16(sizeof(RpGather) * ps.size()), need = gb + tables;
+    if (a.table.n < need) {
+        a.table.free();
+        if (a.table.alloc(2 * need)) return fail(ABG_ENOMEM, "Out of device memory for the history analysis tables");
+    }
+    if (a.h_table_bytes < need) {
+        if (a.h_table) cudaFreeHost(a.h_table);
+        a.h_table_bytes = 0;
+        if (cudaHostAlloc((void**)&a.h_table, 2 * need, cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            a.h_table = nullptr;
+            return fail(ABG_ENOMEM, "Out of page-locked host memory for the history analysis tables");
+        }
+        a.h_table_bytes = 2 * need;
+    }
+    RpGather* g = reinterpret_cast<RpGather*>(a.h_table);
+    unsigned long long max_bytes = 0;
+    for (size_t i = 0; i < ps.size(); i++) {
+        const HiDev& h = e->history.dev[jobs[ps[i].job].dev];
+        g[i] = RpGather{h.ring.p, h.ring.n, ps[i].src, a.scratch.p + ps[i].off, ps[i].bytes};
+        max_bytes = std::max(max_bytes, ps[i].bytes);
+    }
+    fill(a.h_table + gb);
+    const cudaStream_t s = e->stream;
+    CU(cudaMemcpyAsync(a.table.p, a.h_table, need, cudaMemcpyHostToDevice, s));
+    CU(cudaEventRecord(a.ev[0], s));
+    cudaError_t er = abg_launch_replay_gather(reinterpret_cast<const RpGather*>(a.table.p), (int)ps.size(),
+                                              abg_history_blocks(max_bytes, (int)ps.size(), e->sm_count), s);
+    if (er != cudaSuccess) return fail(ABG_ECUDA, "history analysis gather launch failed: %s", cudaGetErrorString(er));
+    e->launches++;
+    CU(cudaEventRecord(a.ev[1], s));
+    er = kernel(a.table.p + gb, s);
+    if (er != cudaSuccess) return fail(ABG_ECUDA, "history analysis %s launch failed: %s", which == 1 ? "spectrum" : "detector", cudaGetErrorString(er));
+    e->launches++;
+    CU(cudaEventRecord(a.ev[2], s));
+    CU(cudaStreamSynchronize(s));
+    float ms = 0.0f;
+    CU(cudaEventElapsedTime(&ms, a.ev[0], a.ev[1]));
+    a.ms[0] += ms;
+    CU(cudaEventElapsedTime(&ms, a.ev[1], a.ev[2]));
+    a.ms[which] += ms;
+    return ABG_OK;
+}
+
+int abg_history_spectrogram(abg_engine* e, int n_jobs, const abg_spectrogram_job* jobs) {
+    if (n_jobs < 1 || n_jobs > 65535 || !jobs)
+        return fail(ABG_EINVAL, "abg_history_spectrogram: %d jobs at %p (1 to 65535)", n_jobs, (const void*)jobs);
+    const int N = e->N;
+    std::vector<AnJob> an(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const abg_spectrogram_job& J = jobs[j];
+        if (!monitor_dev(e, e->history, J.dev, __func__)) return ABG_ERANGE;
+        const int F = J.frames_per_row, s = J.stride;
+        if (J.n_rows < 1 || F < 1 || s < 1 || s > F || !J.power)
+            return fail(ABG_EINVAL, "abg_history_spectrogram: job %d: %d rows of %d frames at stride %d into %p", j, J.n_rows, F, s, (void*)J.power);
+        const int n_sel = (F + s - 1) / s, chunks = (n_sel + ABG_SPEC_FPC - 1) / ABG_SPEC_FPC;
+        an[j] = AnJob{J.dev, J.first_frame, (unsigned long long)F, J.n_rows, n_sel, s, sizeof(float) * N,
+                      chunks > 1 ? sizeof(float) * (size_t)chunks * N : 0};
+        const int rc = analysis_window(e, __func__, j, an[j]);
+        if (rc != ABG_OK) return rc;
+    }
+    auto& a = e->analysis;
+    return analysis_chunks(e, an, [&](const std::vector<AnPiece>& ps) -> int {
+        int rows = 0;
+        for (const AnPiece& p : ps) rows += p.n;
+        const size_t cfg_bytes = align16(sizeof(SpecCfg) * rows);
+        float* ring = nullptr;
+        CU(cudaHostGetDevicePointer((void**)&ring, a.result, 0));
+        int max_items = 0;
+        const int rc = analysis_launch(
+            e, an, ps, cfg_bytes + sizeof(SpecRun) * rows, 1,
+            [&](unsigned char* h) {
+                SpecCfg* hc = reinterpret_cast<SpecCfg*>(h);
+                SpecRun* hr = reinterpret_cast<SpecRun*>(h + cfg_bytes);
+                int32_t* counters = reinterpret_cast<int32_t*>(a.work.p + a.work.n) - kAnalysisMaxUnits;
+                size_t work = 0;
+                int r = 0;
+                // every row is a device of its own with one batch, so the kernel's batch step is never taken
+                for (const AnPiece& p : ps) {
+                    const AnJob& J = an[p.job];
+                    const Device& d = e->dev[J.dev];
+                    for (int u = 0; u < p.n; u++, r++) {
+                        SpecCfg& c = hc[r];
+                        c.wsc = e->groups[d.group].wsc.p;
+                        c.partial = reinterpret_cast<float*>(a.work.p + work);
+                        c.counter = counters + r;
+                        c.ring = ring + (size_t)r * N;
+                        c.hop_bytes = d.hop_bytes; c.sfmt = d.sfmt; c.stride = J.stride; c.n_sel = J.n_sel;
+                        c.n_chunks = (J.n_sel + ABG_SPEC_FPC - 1) / ABG_SPEC_FPC;
+                        c.ring_cap = 1;
+                        work += J.unit_work;
+                        hr[r] = SpecRun{a.scratch.p, p.off + (unsigned long long)u * J.step * d.hop_bytes, 1, 0};
+                        max_items = std::max(max_items, c.n_chunks);
+                    }
+                }
+            },
+            [&](unsigned char* dv, cudaStream_t s) {
+                SpecArgs A{};
+                A.cfg = reinterpret_cast<const SpecCfg*>(dv); A.run = reinterpret_cast<const SpecRun*>(dv + cfg_bytes);
+                A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = 0;
+                return abg_launch_spectrum(N, A, rows, max_items, s);
+            });
+        if (rc != ABG_OK) return rc;
+        const float* res = reinterpret_cast<const float*>(a.result);
+        for (const AnPiece& p : ps) {
+            memcpy(jobs[p.job].power + (size_t)p.u0 * N, res, sizeof(float) * (size_t)p.n * N);
+            res += (size_t)p.n * N;
+        }
+        return ABG_OK;
+    });
+}
+
+// A job's detector pieces joined batch by batch with merge_bursts' rule (lib.py), plus the window's edge flags.  Within a
+// batch, only a bin's first piece can carry OPEN_START and only its last OPEN_END, so the pieces are taken in the order
+// the kernel stored them; the bursts are sorted once at the end.
+struct BurstMerge {
+    struct Open {
+        abg_burst rec;
+        long long q0, q1;  // selected index of its first and last member, counted from the window's start
+        bool live;
+    };
+    std::vector<Open> open, next;      // [fft_size]: per bin the burst that may continue in the next batch
+    std::vector<int32_t> open_bins, next_bins;
+    std::vector<abg_burst> out;
+    int truncated = 0;
+    void keep(const Open& o, int min_span) {
+        if (o.rec.flags != 0 || o.q1 - o.q0 + 1 >= min_span) out.push_back(o.rec);
+    }
+    // batch bi (of n_batches) of the window, its detector entry at `entry`
+    void batch(const abg_activity_job& J, int N, int B, int n_sel, int bi, const unsigned char* entry) {
+        if (open.empty()) open.assign(N, Open{}), next.assign(N, Open{});
+        int32_t head[4];
+        memcpy(head, entry, sizeof(head));
+        const int stored = std::min(head[0], (int32_t)ABG_ACTIVITY_MAX_RECORDS);
+        if (head[0] > ABG_ACTIVITY_MAX_RECORDS) truncated++;
+        const unsigned long long f0 = ABG_AGC_EXTRA + (J.first_batch + (unsigned long long)bi) * B;
+        auto q = [&](uint64_t f) { return (long long)bi * n_sel + (long long)((f - f0) / (unsigned)J.stride); };
+        for (int i = 0; i < stored; i++) {
+            abg_burst p;
+            memcpy(&p, entry + ABG_ACT_HEAD_BYTES + sizeof(abg_burst) * (size_t)i, sizeof(p));
+            Open cur;
+            Open& prev = open[p.bin];
+            if ((p.flags & ABG_BURST_OPEN_START) && prev.live && q(p.first_frame) - prev.q1 <= J.hang + 1) {
+                cur = prev;
+                prev.live = false;
+                cur.rec.last_frame = p.last_frame;
+                cur.rec.n_active += p.n_active;
+                cur.rec.peak = std::max(cur.rec.peak, p.peak);
+                cur.rec.sum = cur.rec.sum + p.sum;
+                cur.q1 = q(p.last_frame);
+            } else {
+                cur.rec = p;
+                cur.rec.flags = bi == 0 && (p.flags & ABG_BURST_OPEN_START) ? ABG_BURST_OPEN_START : 0;
+                cur.q0 = q(p.first_frame);
+                cur.q1 = q(p.last_frame);
+            }
+            cur.live = true;
+            if (p.flags & ABG_BURST_OPEN_END) {
+                next[p.bin] = cur;
+                next_bins.push_back(p.bin);
+            } else {
+                keep(cur, J.min_span);
+            }
+        }
+        for (const int32_t k : open_bins)  // not continued in this batch
+            if (open[k].live) {
+                keep(open[k], J.min_span);
+                open[k].live = false;
+            }
+        open.swap(next);
+        open_bins.swap(next_bins);
+        next_bins.clear();
+        if (bi + 1 < J.n_batches) return;
+        for (const int32_t k : open_bins) {
+            open[k].rec.flags |= ABG_BURST_OPEN_END;
+            out.push_back(open[k].rec);
+            open[k].live = false;
+        }
+        open_bins.clear();
+    }
+};
+
+int abg_history_activity(abg_engine* e, int n_jobs, abg_activity_job* jobs) {
+    if (n_jobs < 1 || n_jobs > 65535 || !jobs)
+        return fail(ABG_EINVAL, "abg_history_activity: %d jobs at %p (1 to 65535)", n_jobs, (const void*)jobs);
+    const int N = e->N, B = e->B;
+    const size_t entry = ABG_ACT_HEAD_BYTES + sizeof(abg_burst) * (size_t)ABG_ACTIVITY_MAX_RECORDS;
+    std::vector<AnJob> an(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        const abg_activity_job& J = jobs[j];
+        if (!monitor_dev(e, e->history, J.dev, __func__)) return ABG_ERANGE;
+        char who[48];
+        snprintf(who, sizeof(who), "abg_history_activity: jobs[%d]", j);
+        int rc = activity_check(e, who, J.stride, J.hang, J.min_span, J.thr);
+        if (rc != ABG_OK) return rc;
+        if (J.stride == 0 || J.n_batches < 1 || J.cap < 0 || (J.cap > 0 && !J.out))
+            return fail(ABG_EINVAL, "%s: stride %d, %d batches, %d bursts into %p", who, J.stride, J.n_batches, J.cap, (void*)J.out);
+        an[j] = AnJob{J.dev, ABG_AGC_EXTRA + (unsigned __int128)J.first_batch * B, (unsigned long long)B, J.n_batches,
+                      (B + J.stride - 1) / J.stride, J.stride, entry, 0};
+        if ((rc = analysis_window(e, __func__, j, an[j])) != ABG_OK) return rc;
+    }
+    auto& a = e->analysis;
+    std::vector<BurstMerge> merge(n_jobs);
+    const int rc = analysis_chunks(e, an, [&](const std::vector<AnPiece>& ps) -> int {
+        const int np = (int)ps.size();
+        const size_t cfg_bytes = align16(sizeof(ActCfg) * np), run_bytes = align16(sizeof(ActRun) * np), thr_bytes = sizeof(float) * N;
+        unsigned char* ring = nullptr;
+        CU(cudaHostGetDevicePointer((void**)&ring, a.result, 0));
+        int max_batches = 0;
+        int rc2 = analysis_launch(
+            e, an, ps, cfg_bytes + run_bytes + thr_bytes * np, 2,
+            [&](unsigned char* h) {
+                ActCfg* hc = reinterpret_cast<ActCfg*>(h);
+                ActRun* hr = reinterpret_cast<ActRun*>(h + cfg_bytes);
+                size_t ent = 0;
+                for (int i = 0; i < np; i++) {
+                    const AnPiece& p = ps[i];
+                    const abg_activity_job& J = jobs[p.job];
+                    const Device& d = e->dev[J.dev];
+                    memcpy(h + cfg_bytes + run_bytes + thr_bytes * i, J.thr, thr_bytes);
+                    ActCfg& c = hc[i];
+                    c.wsc = e->groups[d.group].wsc.p;
+                    c.thr = reinterpret_cast<const float*>(a.table.p + align16(sizeof(RpGather) * ps.size()) + cfg_bytes + run_bytes + thr_bytes * i);
+                    c.ring = ring + ent * entry;
+                    c.hop_bytes = d.hop_bytes; c.sfmt = d.sfmt; c.stride = J.stride; c.n_sel = an[p.job].n_sel;
+                    c.hang = J.hang; c.min_span = J.min_span; c.ring_cap = p.n; c.entry_bytes = (int32_t)entry;
+                    hr[i] = ActRun{a.scratch.p, p.off, (unsigned long long)ABG_AGC_EXTRA + (J.first_batch + (unsigned long long)p.u0) * B, p.n, 0};
+                    ent += p.n;
+                    max_batches = std::max(max_batches, p.n);
+                }
+            },
+            [&](unsigned char* dv, cudaStream_t s) {
+                ActArgs A{};
+                A.cfg = reinterpret_cast<const ActCfg*>(dv); A.run = reinterpret_cast<const ActRun*>(dv + cfg_bytes);
+                A.tw1 = e->tw1.p; A.tw2 = e->tw2.p; A.wave_batch = B;
+                return abg_launch_activity(N, A, np, max_batches, s);
+            });
+        if (rc2 != ABG_OK) return rc2;
+        const unsigned char* res = a.result;
+        for (const AnPiece& p : ps)
+            for (int b = 0; b < p.n; b++, res += entry) merge[p.job].batch(jobs[p.job], N, B, an[p.job].n_sel, p.u0 + b, res);
+        return ABG_OK;
+    });
+    if (rc != ABG_OK) return rc;
+    for (int j = 0; j < n_jobs; j++) {
+        std::vector<abg_burst>& v = merge[j].out;
+        std::sort(v.begin(), v.end(), [](const abg_burst& x, const abg_burst& y) {
+            return x.bin != y.bin ? x.bin < y.bin : x.first_frame < y.first_frame;
+        });
+        if (jobs[j].cap > 0) memcpy(jobs[j].out, v.data(), sizeof(abg_burst) * std::min(v.size(), (size_t)jobs[j].cap));
+        jobs[j].n_bursts = (int32_t)v.size();
+        jobs[j].n_truncated = merge[j].truncated;
+    }
+    return ABG_OK;
+}
+
+int abg_debug_history_analysis_time(abg_engine* e, float* ms3) {
+    if (!ms3) return fail(ABG_EINVAL, "abg_debug_history_analysis_time: null argument");
+    memcpy(ms3, e->analysis.ms, sizeof(e->analysis.ms));
     return ABG_OK;
 }
 

@@ -33,6 +33,7 @@ SYMBOLS = [
     "abg_history_replay", "abg_debug_replay_time",
     "abg_follow_open", "abg_follow_close", "abg_follow_run", "abg_follow_fetch", "abg_follow_info", "abg_follow_stats",
     "abg_debug_follow_time",
+    "abg_history_spectrogram", "abg_history_activity", "abg_debug_history_analysis_time",
 ]
 
 SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
@@ -111,6 +112,36 @@ class CFollowStatus(C.Structure):
         ("next_batch", C.c_uint64),
         ("queued", C.c_int32),
         ("lost", C.c_int32),
+    ]
+
+
+class CSpectrogramJob(C.Structure):
+    """abg_spectrogram_job: one history spectrogram job (definition in airband_b200.h)."""
+    _fields_ = [
+        ("dev", C.c_int32),
+        ("n_rows", C.c_int32),
+        ("first_frame", C.c_uint64),
+        ("frames_per_row", C.c_int32),
+        ("stride", C.c_int32),
+        ("power", C.c_void_p),
+    ]
+
+
+class CActivityJob(C.Structure):
+    """abg_activity_job: one history activity job (definition in airband_b200.h); n_bursts and n_truncated are written
+    back."""
+    _fields_ = [
+        ("dev", C.c_int32),
+        ("n_batches", C.c_int32),
+        ("first_batch", C.c_uint64),
+        ("stride", C.c_int32),
+        ("hang", C.c_int32),
+        ("min_span", C.c_int32),
+        ("cap", C.c_int32),
+        ("thr", C.c_void_p),
+        ("out", C.c_void_p),
+        ("n_bursts", C.c_int32),
+        ("n_truncated", C.c_int32),
     ]
 
 
@@ -218,6 +249,9 @@ def load():
     L.abg_follow_info.restype, L.abg_follow_info.argtypes = i, [vp, C.c_int32, C.POINTER(CFollowStatus)]
     L.abg_follow_stats.restype, L.abg_follow_stats.argtypes = i, [vp, C.c_int32, i, C.POINTER(CSquelchStats)]
     L.abg_debug_follow_time.restype, L.abg_debug_follow_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_history_spectrogram.restype, L.abg_history_spectrogram.argtypes = i, [vp, i, C.POINTER(CSpectrogramJob)]
+    L.abg_history_activity.restype, L.abg_history_activity.argtypes = i, [vp, i, C.POINTER(CActivityJob)]
+    L.abg_debug_history_analysis_time.restype, L.abg_debug_history_analysis_time.argtypes = i, [vp, C.POINTER(C.c_float)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -661,6 +695,53 @@ class Engine:
         ms = (C.c_float * 2)()
         self._chk(self.L.abg_debug_follow_time(self.h, ms))
         return float(ms[0]), float(ms[1])
+
+    # ---- history analysis -----------------------------------------------------------------------------------------
+    def history_spectrogram(self, jobs) -> List[np.ndarray]:
+        """Band spectra of windows of the history, all jobs in one call (definition in airband_b200.h).  jobs: dicts with
+        dev, first_frame, n_rows, stride and frames_per_row (default wave_batch); with frames_per_row = wave_batch and
+        first_frame = AGC_EXTRA + b * wave_batch, row r is bitwise the live spectrum of batch b + r.  Returns per job
+        float32[n_rows, fft_size].  history_window gives a window the history holds."""
+        arr = (CSpectrogramJob * max(len(jobs), 1))()
+        out = []
+        for k, j in enumerate(jobs):
+            p = np.zeros((max(int(j["n_rows"]), 0), self.cfg.fft_size), np.float32)
+            arr[k] = CSpectrogramJob(int(j["dev"]), int(j["n_rows"]), int(j["first_frame"]), int(j.get("frames_per_row", self.B)),
+                                     int(j["stride"]), _ptr(p))
+            out.append(p)
+        self._chk(self.L.abg_history_spectrogram(self.h, len(jobs), arr))
+        return out
+
+    def history_activity(self, jobs) -> List[dict]:
+        """The activity detector over windows of the history, all jobs in one call (definition in airband_b200.h).  jobs:
+        dicts with dev, first_batch, n_batches, stride, thr[fft_size], hang (default 0) and min_span (default 1).
+        Returns per job a dict of bursts (BURST_DTYPE, sorted by (bin, first_frame): merge_bursts of the live readings,
+        with OPEN_START / OPEN_END on the bursts at the window's edges, kept whatever their span) and n_truncated (batches
+        whose pieces did not all fit a reading; their bursts are unspecified)."""
+        def call(caps):
+            arr = (CActivityJob * max(len(jobs), 1))()
+            keep = []
+            for k, j in enumerate(jobs):
+                t = np.ascontiguousarray(j["thr"], dtype=np.float32)
+                b = np.zeros(caps[k], BURST_DTYPE)
+                keep.append((t, b))
+                arr[k] = CActivityJob(int(j["dev"]), int(j["n_batches"]), int(j["first_batch"]), int(j["stride"]), int(j.get("hang", 0)),
+                                      int(j.get("min_span", 1)), caps[k], _ptr(t), _ptr(b) if caps[k] else None, 0, 0)
+            self._chk(self.L.abg_history_activity(self.h, len(jobs), arr))
+            return arr, keep
+
+        caps = [4096] * len(jobs)
+        arr, keep = call(caps)
+        if any(arr[k].n_bursts > caps[k] for k in range(len(jobs))):  # the results do not depend on the call: repeat with room
+            arr, keep = call([max(caps[k], arr[k].n_bursts) for k in range(len(jobs))])
+        return [dict(bursts=keep[k][1][:arr[k].n_bursts].copy(), n_truncated=int(arr[k].n_truncated)) for k in range(len(jobs))]
+
+    def history_analysis_time(self) -> Tuple[float, float, float]:
+        """(gather ms, spectrum kernel ms, detector kernel ms) of the most recent history_spectrogram or history_activity,
+        summed over its chunks, from CUDA events; 0 where it had none."""
+        ms = (C.c_float * 3)()
+        self._chk(self.L.abg_debug_history_analysis_time(self.h, ms))
+        return float(ms[0]), float(ms[1]), float(ms[2])
 
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
@@ -1107,3 +1188,45 @@ def transmission_follow(tx: dict, cfg: Config, dev: int, history_range: Tuple[in
     b0, _ = _lead_in_batch(tx, cfg, dev, history_range, lead_s, "transmission_follow")
     ch = make_channel(int(round(tx["freq_hz"])), d.centerfreq, d.sample_rate, cfg.fft_size, cfg.wave_rate, **channel_kw)
     return dict(dev=dev, first_batch=b0, channels=[ch])
+
+
+def history_window(cfg: Config, dev: int, history_range: Tuple[int, int], stride: int = 1, frames_per_row: Optional[int] = None,
+                   seconds: Optional[float] = None) -> Tuple[int, int]:
+    """The longest window of device dev that the history (history_range = (first, end), Engine.history_range) fully holds
+    for history analysis at this stride, with the engine's rule: every sample of every selected frame lies in [first, end).
+    frames_per_row None: the detector's window, whole batches, returned as (first_batch, n_batches).  frames_per_row F: a
+    spectrogram's window of F-frame rows on the grid of rows that start at frame AGC_EXTRA + k * F (with F = wave_batch, the
+    batches), returned as (first_frame, n_rows).  seconds: only the newest units that cover at least that long.  Raises
+    ValueError if not one unit fits."""
+    B, hop, N = cfg.wave_batch, cfg.hop(dev), cfg.fft_size
+    step = B if frames_per_row is None else int(frames_per_row)
+    if stride < 1 or step < 1 or stride > step:
+        raise ValueError(f"history_window: stride {stride} must be in [1, {step}]")
+    n_sel = -(-step // stride)
+    first, end = (int(x) for x in history_range)
+    # unit k reads the samples [(AGC_EXTRA + k*step) * hop, (AGC_EXTRA + k*step + (n_sel - 1) * stride) * hop + N)
+    k_lo = max(0, -(-(-(-first // hop) - AGC_EXTRA) // step))
+    k_hi = ((end - N) // hop - (n_sel - 1) * stride - AGC_EXTRA) // step  # inclusive
+    n = k_hi - k_lo + 1
+    if seconds is not None:
+        n = min(n, max(1, int(np.ceil(seconds * cfg.devices[dev].sample_rate / (step * hop)))))
+        k_lo = k_hi - n + 1
+    if end <= first or n < 1:
+        raise ValueError(f"history_window: no {'batch' if frames_per_row is None else 'row'} of {step} frames at stride {stride} "
+                         f"fits the history [{first}, {end})")
+    return (k_lo, n) if frames_per_row is None else (AGC_EXTRA + k_lo * step, n)
+
+
+def history_transmissions(e: Engine, cfg: Config, dev: int, margin_db: float, half_width: int, stride: int, hang: int = 0,
+                          min_span: int = 1, seconds: Optional[float] = None, max_bin_gap: int = 1) -> List[dict]:
+    """What transmitted on device dev during the window its history holds (the newest `seconds` of it, if given), with
+    nothing configured in advance but the history: a spectrogram of the window's batches at `stride` (Engine.
+    history_spectrogram, F = wave_batch), thresholds from it (activity_threshold(margin_db, half_width)), the detector
+    over the same batches (Engine.history_activity with stride, hang and min_span), and the bursts grouped
+    (group_transmissions).  Returns group_transmissions' list, which transmission_replay and transmission_follow take."""
+    b0, nb = history_window(cfg, dev, e.history_range(dev), stride=stride, seconds=seconds)
+    B = cfg.wave_batch
+    spec = e.history_spectrogram([dict(dev=dev, first_frame=AGC_EXTRA + b0 * B, n_rows=nb, frames_per_row=B, stride=stride)])[0]
+    thr = activity_threshold(spec, margin_db, half_width)
+    act = e.history_activity([dict(dev=dev, first_batch=b0, n_batches=nb, stride=stride, hang=hang, min_span=min_span, thr=thr)])[0]
+    return group_transmissions(act["bursts"], cfg, dev, max_bin_gap=max_bin_gap)
