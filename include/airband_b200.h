@@ -679,6 +679,81 @@ ABG_API int abg_history_activity(abg_engine* e, int n_jobs, abg_activity_job* jo
  * ms3[0] = its gathers, ms3[1] = its spectrum kernels, ms3[2] = its detector kernels; 0 where it had none. */
 ABG_API int abg_debug_history_analysis_time(abg_engine* e, float* ms3);
 
+/* Transmission profiles (not part of the reference surface: replaying or following a transmission the activity detector
+ * found needs its modulation and CTCSS tone, and a frequency better than the detector's bin; the carrier and tone meters
+ * only read configured channels, and the tone meter reads gated audio).  A profile is measured on the raw baseband,
+ * before any demodulation.
+ * A job names dev, a down-converter (offset_hz, decimation D, coefficients h[0..L)), checked as abg_history_subband checks
+ * them, an output window m in [m0, m0 + n), n >= 2, and a tone list f_k, k < K <= ABG_TONE_MAX, each finite and in
+ * (0, fs_out / 2) with fs_out = sample_rate / D (tones == NULL or n_tones == 0: the 51 standard tones).  y[m] is bitwise what
+ * abg_history_subband(dev, offset_hz, D, L, h, m0, n) returns; then, in float32:
+ *     p[m]   = fmaf(y.re, y.re, y.im * y.im)          a[m] = sqrtf(p[m])
+ *     z[m]   = y[m+1] * conj(y[m]):  z.re = fmaf(y1.re, y0.re, y1.im * y0.im),  z.im = fmaf(y1.im, y0.re, -(y1.re * y0.im))
+ *     phi[m] = atan2f(z.im, z.re)                     for m < m0 + n - 1 (the n - 1 pairs)
+ *     delta_k = llround(f_k / fs_out * 2^32) mod 2^32 (the tone meter's integer phase, on the absolute output index m);
+ *     c + i s = the float32 cospi / sinpi (sincospif) of (float)(int32_t)(delta_k * m mod 2^32) * 2^-31
+ *     tone_fm[k] += (fmaf(phi, c, .), fmaf(-phi, s, .))    tone_am[k] += (fmaf(a, c, .), fmaf(-a, s, .))
+ * and the reading holds n, p1 = sum p, p2 = sum p^2 (fmaf(p, p, .)), a1 = sum a, z = sum z, f1 = sum phi, f2 = sum phi^2
+ * (fmaf(phi, phi, .)), tone_fm[k] = sum phi[m] exp(-2 pi i ((delta_k m) mod 2^32) / 2^32), tone_am[k] the same sum of a[m]
+ * (a phi of an output without a successor counts as 0), and n_tones = K.  Meaning: arg(z) * fs_out / 2 pi is the carrier's
+ * offset from the down-converter's true frequency (lib.subband_frequency); f2 about the mean f1 / (n - 1) gives the FM
+ * deviation; n * p2 / p1^2 - 1 the envelope's spread; the tone sums carry a CTCSS tone in NFM (tone_fm) and AM (tone_am).
+ * Order: the outputs are cut into blocks of ABG_PROFILE_BLOCK outputs (and their pairs) anchored at m0.  Within a block,
+ * thread t of 256 adds the terms of outputs t, t + 256, t + 512, t + 768 in that order and a fixed xor-shuffle tree and the
+ * 8 warps in order add those; a tone sum is added by lane l over l, l + 32, ... in order, then by the xor tree.  The host
+ * adds the block sums in double, in block order.  A reading is therefore bitwise reproducible for any grouping of jobs
+ * into calls, job order, chunking, max_batches_per_run, push pattern and set of live monitors.
+ * Bound: against float64 sums of the same float32 terms with the exact phase, each of p1, p2, a1, z, f1, f2 is within
+ * 16 * 2^-24 * sum |term| (15 float32 roundings per term at most, then the double sum), and each component of a tone sum
+ * within 40 * 2^-24 * sum |x| (x = phi or a: 37 roundings at most, the phase's rounding to float, pi * 2^-25, and
+ * sincospif's 1 ulp).
+ * Window: every tap of every output must lie in abg_history_range, by abg_history_subband's rule: ABG_ERANGE when it does
+ * not (the message gives the needed range), when the history is off, and for a bad dev; ABG_EINVAL for n_jobs outside
+ * [1, 65535], a null jobs or out, n < 2 and a bad tone list.  The call waits for its results.
+ * Computed on the GPU: per chunk, one launch of the history capture per job piece writes y into the profile's own scratch
+ * (one extra output at a seam, so that the pair across it is formed from captured values), then one launch of the profile
+ * kernel covers every block of every job of the chunk, one CTA per block; the block sums go to a results buffer the host
+ * reads after the chunk.  Chunks hold at most 8 M outputs of scratch and 65535 blocks.  Everything runs on the K1 stream,
+ * behind every append it reads.  Nothing is allocated before the first call; everything is freed when the last history is
+ * switched off and by abg_destroy.  Live runs launch nothing new. */
+#define ABG_PROFILE_BLOCK 1024
+typedef struct abg_profile {
+    int64_t n;                          /* outputs */
+    int32_t n_tones;                    /* K */
+    int32_t reserved;                   /* 0 */
+    double p1, p2, a1;
+    double z[2];
+    double f1, f2;
+    double tone_fm[ABG_TONE_MAX][2];    /* [K][re, im] */
+    double tone_am[ABG_TONE_MAX][2];
+} abg_profile;
+typedef struct abg_profile_job {
+    int32_t dev;
+    int32_t decim;                      /* D, 1 .. WAVE_BATCH * hop */
+    double offset_hz;
+    int32_t n_coeffs;                   /* L, 1 .. ABG_SUBBAND_MAX_COEFFS */
+    int32_t n_tones;                    /* K, 0 .. ABG_TONE_MAX (0: the 51 standard tones) */
+    const float* coeffs;                /* h[L] */
+    uint64_t first_m;                   /* m0 */
+    int64_t n_out;                      /* n >= 2 */
+    const float* tones;                 /* f_k [K] in Hz, or NULL */
+    abg_profile* out;                   /* written */
+} abg_profile_job;
+ABG_API int abg_history_profile(abg_engine* e, int n_jobs, abg_profile_job* jobs);
+/* Measurement aid: device time of the most recent abg_history_profile, summed over its chunks: ms2[0] = its capture
+ * kernels, ms2[1] = its profile kernels; 0 before the first. */
+ABG_API int abg_debug_history_profile_time(abg_engine* e, float* ms2);
+/* Host-only: the chunk and block plan abg_history_profile launches for jobs of these shapes (first_m, n_out, n_coeffs and
+ * n_tones as in abg_profile_job, n_tones already resolved, 1 .. ABG_TONE_MAX), without an engine.  limits[4] = {scratch
+ * outputs, blocks, result floats, coefficients} per chunk.  pieces[cap_pieces][6] = {chunk, job, first output captured,
+ * outputs captured, scratch offset, coefficient offset}: one capture launch each, in launch order.  blocks[cap_blocks][8] =
+ * {chunk, job, piece, scratch offset, first output, outputs, successor (0 / 1), result offset}: one CTA each.  *n_pieces
+ * and *n_blocks are always written; rows past a cap are not.  ABG_EINVAL for what abg_history_profile refuses of these
+ * fields. */
+ABG_API int abg_debug_profile_plan(int n_jobs, const uint64_t* first_m, const int64_t* n_out, const int32_t* n_coeffs,
+                                   const int32_t* n_tones, int64_t* limits, int64_t* pieces, int cap_pieces, int32_t* n_pieces,
+                                   int64_t* blocks, int cap_blocks, int32_t* n_blocks);
+
 /* Mixer path (reference src/mixer.cpp:82-83,114-140,189-214): mixer m's output for a batch is, per sample,
  * sum over its inputs (in input order) of waveout * (ampfactor * ampl) [left] and * (ampfactor * ampr) [right], taken
  * over the inputs whose channel had axcindicate != NO_SIGNAL in that batch (mixer_put_samples' has_signal), where

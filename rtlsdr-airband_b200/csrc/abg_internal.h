@@ -333,6 +333,25 @@ struct HiCapture {  // one capture launch: outputs [m0, m0 + n_out) of one devic
 };
 cudaError_t abg_launch_history_capture(HiCapture c, cudaStream_t s);
 
+// transmission profiles (profile.cu): see abg_history_profile in include/airband_b200.h
+#define ABG_PROFILE_SUMS 8  // p1, p2, a1, z.re, z.im, f1, f2, 0; then tone_fm[K][2], tone_am[K][2]
+struct ProfBlock {  // one CTA: every device read it makes is bounded by its own fields
+    unsigned long long off;  // scratch index of y[m]
+    unsigned long long res;  // result index (floats) of its ABG_PROFILE_SUMS + 4 K sums
+    long long m;             // absolute output index of its first output
+    int32_t n;               // outputs, 1 .. ABG_PROFILE_BLOCK
+    int32_t succ;            // 1: y[m + n] is captured at off + n, so the pair of its last output is formed
+    int32_t tones;           // index of its delta_0 in the delta table
+    int32_t K;               // tones, 1 .. ABG_TONE_MAX
+};
+struct ProfArgs {
+    const float2* y;         // the chunk's captured outputs
+    const ProfBlock* blocks;   // [n_blocks]
+    const uint32_t* delta;   // the chunk's tone phases
+    float* res;              // block sums
+};
+cudaError_t abg_launch_profile(const ProfArgs& a, int n_blocks, cudaStream_t s);
+
 // history replay (replay.cu): see abg_history_replay in include/airband_b200.h
 struct RpGather {  // one job's bytes of one chunk
     const unsigned char* ring;       // the parent device's history ring: stream byte b at b mod ring_bytes

@@ -605,6 +605,17 @@ struct abg_engine {
         cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // gather start, gather end, kernel end
         float ms[3] = {0.0f, 0.0f, 0.0f};  // the latest call: gathers, spectrum kernels, detector kernels
     } analysis;
+    // transmission profiles (abg_history_profile): the call's own buffers; created by the first call, freed when the last
+    // history is switched off
+    struct Profile {
+        DevBuf<float2> scratch;            // one chunk's captured outputs
+        DevBuf<unsigned char> table;       // one chunk's coefficients, tone phases and block table
+        DevBuf<float> res;                 // one chunk's block sums
+        unsigned char* h_table = nullptr;  // page-locked staging of `table`
+        float* h_res = nullptr;            // page-locked copy of `res`
+        cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};  // captures start, captures end, profile kernel end
+        float ms[2] = {0.0f, 0.0f};        // the latest call: captures, profile kernels
+    } profile;
 
     K2Launch k2_launch(int cur) const {
         K2Launch L{};
@@ -786,6 +797,22 @@ void analysis_free(abg_engine* e) {
     }
 }
 
+// The transmission profile buffers and events (abg_history_profile).
+void profile_free(abg_engine* e) {
+    auto& p = e->profile;
+    p.scratch.free();
+    p.table.free();
+    p.res.free();
+    if (p.h_table) cudaFreeHost(p.h_table);
+    if (p.h_res) cudaFreeHost(p.h_res);
+    p.h_table = nullptr;
+    p.h_res = nullptr;
+    for (auto& ev : p.ev) {
+        if (ev) cudaEventDestroy(ev);
+        ev = nullptr;
+    }
+}
+
 void engine_free(abg_engine* e) {
     if (!e) return;
     cudaSetDevice(e->cuda_dev);
@@ -794,6 +821,7 @@ void engine_free(abg_engine* e) {
     replay_free(e);
     follow_free(e);
     analysis_free(e);
+    profile_free(e);
     for (auto& d : e->dev) {
         for (int i = 0; i < 2; i++)
             if (d.raw[i]) cudaFree(d.raw[i]);
@@ -2272,6 +2300,7 @@ int abg_history_configure(abg_engine* e, int dev, int n_batches) {
         replay_free(e);
         follow_free(e);
         analysis_free(e);
+        profile_free(e);
     }
     return rc != ABG_OK ? rc : rp;
 }
@@ -3314,6 +3343,292 @@ int abg_history_activity(abg_engine* e, int n_jobs, abg_activity_job* jobs) {
 int abg_debug_history_analysis_time(abg_engine* e, float* ms3) {
     if (!ms3) return fail(ABG_EINVAL, "abg_debug_history_analysis_time: null argument");
     memcpy(ms3, e->analysis.ms, sizeof(e->analysis.ms));
+    return ABG_OK;
+}
+
+// ---- transmission profiles (definition in airband_b200.h) ----------------------------------------------------------------
+// A job's outputs are cut into blocks of ABG_PROFILE_BLOCK anchored at its m0; a call is cut into chunks of whole blocks,
+// in job and block order, within fixed budgets.  A chunk holds one piece per job it touches: the piece's consecutive
+// blocks, captured by one launch of the history capture into the scratch, plus the output after its last block when the
+// job goes on (the successor of the pair across the seam).  The plan is a pure host function, so that every index the
+// kernel reads can be checked without a GPU (abg_debug_profile_plan).
+constexpr long long kProfileScratch = 8ll << 20;  // captured outputs per chunk: 64 MB of float2, the analysis figure
+constexpr int kProfileBlocks = 65535;             // CTAs of a profile launch
+constexpr long long kProfileResult = 8ll << 20;   // block sums per chunk (floats): 32 MB
+constexpr long long kProfileCoeffs = 2ll << 20;   // capture coefficients per chunk (float2): 16 MB
+
+static_assert(sizeof(abg_profile) == 2120 && sizeof(abg_profile_job) == 64, "the profile structs have a fixed layout");
+
+struct ProfShape {  // what the plan needs of a job
+    unsigned long long m0;
+    long long n;
+    int L, K;
+};
+struct ProfPiece {  // one capture: outputs [m, m + count) of job `job` at scratch index off
+    int chunk, job;
+    unsigned long long m;
+    long long count;
+    unsigned long long off, coef, tones;  // scratch index; index of its g[0] and its delta_0 in the chunk's tables
+};
+struct ProfPlanned {
+    int chunk, job, piece;
+    ProfBlock b;
+};
+
+static void profile_plan(const std::vector<ProfShape>& jobs, std::vector<ProfPiece>& pieces, std::vector<ProfPlanned>& blocks) {
+    constexpr long long PB = ABG_PROFILE_BLOCK;
+    int chunk = 0, nb = 0;
+    long long scratch = 0, res = 0, coef = 0, tones = 0;
+    for (int j = 0; j < (int)jobs.size(); j++) {
+        const ProfShape& J = jobs[j];
+        const long long nblk = (J.n + PB - 1) / PB, rb = ABG_PROFILE_SUMS + 4ll * J.K;
+        for (long long k = 0; k < nblk; k++) {
+            const unsigned long long m = J.m0 + (unsigned long long)(k * PB);
+            const long long cnt = std::min(PB, J.n - k * PB);
+            const int succ = k + 1 < nblk ? 1 : 0;
+            for (;;) {
+                const bool extend = !pieces.empty() && pieces.back().chunk == chunk && pieces.back().job == j;
+                // extending: the previous block of the piece had a successor, which is this block's first output
+                const long long s_need = extend ? (long long)pieces.back().off + pieces.back().count - 1 + cnt + succ : scratch + cnt + succ;
+                const long long c_need = coef + (extend ? 0 : J.L), t_need = tones + (extend ? 0 : J.K);
+                const bool fits = s_need <= kProfileScratch && nb < kProfileBlocks && res + rb <= kProfileResult && c_need <= kProfileCoeffs;
+                if (!fits && nb > 0) {  // (a block alone always fits)
+                    chunk++;
+                    nb = 0;
+                    scratch = res = coef = tones = 0;
+                    continue;
+                }
+                if (extend) {
+                    pieces.back().count += cnt + succ - 1;
+                } else {
+                    pieces.push_back(ProfPiece{chunk, j, m, cnt + succ, (unsigned long long)scratch, (unsigned long long)coef, (unsigned long long)tones});
+                    coef = c_need;
+                    tones = t_need;
+                }
+                const ProfPiece& p = pieces.back();
+                scratch = s_need;
+                blocks.push_back(ProfPlanned{chunk, j, (int)pieces.size() - 1,
+                                           ProfBlock{p.off + (m - p.m), (unsigned long long)res, (long long)m, (int32_t)cnt, succ, (int32_t)p.tones, J.K}});
+                res += rb;
+                nb++;
+                break;
+            }
+        }
+    }
+}
+
+// The shape fields of a job as abg_history_profile checks them.
+static int profile_shape_check(const char* who, long long n, int L, int K) {
+    if (n < 2) return fail(ABG_EINVAL, "%s: %lld outputs (at least 2)", who, n);
+    if (L < 1 || L > ABG_SUBBAND_MAX_COEFFS) return fail(ABG_EINVAL, "%s: %d coefficients outside [1, %d]", who, L, ABG_SUBBAND_MAX_COEFFS);
+    if (K < 1 || K > ABG_TONE_MAX) return fail(ABG_EINVAL, "%s: %d tones outside [1, %d]", who, K, ABG_TONE_MAX);
+    return ABG_OK;
+}
+
+int abg_debug_profile_plan(int n_jobs, const uint64_t* first_m, const int64_t* n_out, const int32_t* n_coeffs, const int32_t* n_tones,
+                           int64_t* limits, int64_t* pieces, int cap_pieces, int32_t* n_pieces, int64_t* blocks, int cap_blocks,
+                           int32_t* n_blocks) {
+    if (n_jobs < 1 || n_jobs > 65535 || !first_m || !n_out || !n_coeffs || !n_tones || !n_pieces || !n_blocks)
+        return fail(ABG_EINVAL, "abg_debug_profile_plan: %d jobs (1 to 65535) or a null argument", n_jobs);
+    std::vector<ProfShape> shapes(n_jobs);
+    for (int j = 0; j < n_jobs; j++) {
+        char who[48];
+        snprintf(who, sizeof(who), "abg_debug_profile_plan: jobs[%d]", j);
+        const int rc = profile_shape_check(who, n_out[j], n_coeffs[j], n_tones[j]);
+        if (rc != ABG_OK) return rc;
+        shapes[j] = ProfShape{first_m[j], n_out[j], n_coeffs[j], n_tones[j]};
+    }
+    std::vector<ProfPiece> ps;
+    std::vector<ProfPlanned> bs;
+    profile_plan(shapes, ps, bs);
+    if (limits) {
+        const int64_t lim[4] = {kProfileScratch, kProfileBlocks, kProfileResult, kProfileCoeffs};
+        memcpy(limits, lim, sizeof(lim));
+    }
+    *n_pieces = (int32_t)ps.size();
+    *n_blocks = (int32_t)bs.size();
+    for (int i = 0; pieces && i < (int)ps.size() && i < cap_pieces; i++) {
+        const ProfPiece& p = ps[i];
+        const int64_t row[6] = {p.chunk, p.job, (int64_t)p.m, p.count, (int64_t)p.off, (int64_t)p.coef};
+        memcpy(pieces + 6 * (size_t)i, row, sizeof(row));
+    }
+    for (int i = 0; blocks && i < (int)bs.size() && i < cap_blocks; i++) {
+        const ProfPlanned& q = bs[i];
+        const int64_t row[8] = {q.chunk, q.job, q.piece, (int64_t)q.b.off, q.b.m, q.b.n, q.b.succ, (int64_t)q.b.res};
+        memcpy(blocks + 8 * (size_t)i, row, sizeof(row));
+    }
+    return ABG_OK;
+}
+
+// One chunk: pieces [p0, p1) and blocks [b0, b1) of the plan.  On the K1 stream: the upload of its tables, one capture
+// per piece into the scratch (behind every append it reads, ahead of every later one that would overwrite its samples),
+// the profile kernel, and the copy of the block sums; waits for them.
+static int profile_chunk(abg_engine* e, const abg_profile_job* jobs, const std::vector<uint32_t>& tdelta, const std::vector<ProfPiece>& ps,
+                         size_t p0, size_t p1, const std::vector<ProfPlanned>& bs, size_t b0, size_t b1) {
+    auto& P = e->profile;
+    const ProfPiece& last = ps[p1 - 1];
+    const size_t n_coef = last.coef + jobs[last.job].n_coeffs, n_delta = last.tones + tdelta[(size_t)last.job * (ABG_TONE_MAX + 1)];
+    const size_t coef_bytes = align16(sizeof(float2) * n_coef), delta_bytes = align16(sizeof(uint32_t) * n_delta);
+    const size_t need = coef_bytes + delta_bytes + sizeof(ProfBlock) * (b1 - b0);
+    if (P.table.n < need) {
+        P.table.free();
+        if (P.table.alloc(2 * need)) return fail(ABG_ENOMEM, "Out of device memory for the transmission profile tables");
+        if (P.h_table) cudaFreeHost(P.h_table);
+        if (cudaHostAlloc((void**)&P.h_table, 2 * need, cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            P.h_table = nullptr;
+            P.table.free();
+            return fail(ABG_ENOMEM, "Out of page-locked host memory for the transmission profile tables");
+        }
+    }
+    float2* hc = reinterpret_cast<float2*>(P.h_table);
+    uint32_t* hd = reinterpret_cast<uint32_t*>(P.h_table + coef_bytes);
+    ProfBlock* hb = reinterpret_cast<ProfBlock*>(P.h_table + coef_bytes + delta_bytes);
+    std::vector<float2> g;
+    std::vector<uint32_t> sb_delta(p1 - p0);
+    for (size_t i = p0; i < p1; i++) {
+        const abg_profile_job& J = jobs[ps[i].job];
+        sb_delta[i - p0] = subband_coefficients(J.offset_hz, e->dev[J.dev].sample_rate, J.n_coeffs, J.coeffs, g);
+        memcpy(hc + ps[i].coef, g.data(), sizeof(float2) * J.n_coeffs);
+        const uint32_t* td = &tdelta[(size_t)ps[i].job * (ABG_TONE_MAX + 1)];
+        memcpy(hd + ps[i].tones, td + 1, sizeof(uint32_t) * td[0]);
+    }
+    unsigned long long res_floats = 0;
+    for (size_t i = b0; i < b1; i++) {
+        hb[i - b0] = bs[i].b;
+        res_floats = std::max(res_floats, bs[i].b.res + ABG_PROFILE_SUMS + 4ull * bs[i].b.K);
+    }
+    const cudaStream_t s = e->stream;
+    CU(cudaMemcpyAsync(P.table.p, P.h_table, need, cudaMemcpyHostToDevice, s));
+    CU(cudaEventRecord(P.ev[0], s));
+    for (size_t i = p0; i < p1; i++) {
+        const ProfPiece& p = ps[i];
+        const abg_profile_job& J = jobs[p.job];
+        const Device& d = e->dev[J.dev];
+        const HiDev& h = e->history.dev[J.dev];
+        HiCapture c{};
+        c.ring = h.ring.p; c.ring_bytes = h.ring.n; c.coef = reinterpret_cast<const float2*>(P.table.p) + p.coef;
+        c.out = P.scratch.p + p.off; c.m0 = (long long)p.m; c.n_out = (int32_t)p.count;
+        c.decim = J.decim; c.n_coeffs = J.n_coeffs; c.sfmt = d.sfmt; c.delta = sb_delta[i - p0]; c.scale = 1.0f / d.fullscale;
+        const cudaError_t er = abg_launch_history_capture(c, s);
+        if (er != cudaSuccess) return fail(ABG_ECUDA, "transmission profile capture launch failed: %s", cudaGetErrorString(er));
+        e->launches++;
+    }
+    CU(cudaEventRecord(P.ev[1], s));
+    ProfArgs A{};
+    A.y = P.scratch.p; A.blocks = reinterpret_cast<const ProfBlock*>(P.table.p + coef_bytes + delta_bytes);
+    A.delta = reinterpret_cast<const uint32_t*>(P.table.p + coef_bytes); A.res = P.res.p;
+    const cudaError_t er = abg_launch_profile(A, (int)(b1 - b0), s);
+    if (er != cudaSuccess) return fail(ABG_ECUDA, "transmission profile launch failed: %s", cudaGetErrorString(er));
+    e->launches++;
+    CU(cudaEventRecord(P.ev[2], s));
+    CU(cudaMemcpyAsync(P.h_res, P.res.p, sizeof(float) * res_floats, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    float ms = 0.0f;
+    CU(cudaEventElapsedTime(&ms, P.ev[0], P.ev[1]));
+    P.ms[0] += ms;
+    CU(cudaEventElapsedTime(&ms, P.ev[1], P.ev[2]));
+    P.ms[1] += ms;
+    return ABG_OK;
+}
+
+int abg_history_profile(abg_engine* e, int n_jobs, abg_profile_job* jobs) {
+    if (n_jobs < 1 || n_jobs > 65535 || !jobs)
+        return fail(ABG_EINVAL, "abg_history_profile: %d jobs at %p (1 to 65535)", n_jobs, (const void*)jobs);
+    std::vector<ProfShape> shapes(n_jobs);
+    std::vector<uint32_t> tdelta((size_t)n_jobs * (ABG_TONE_MAX + 1));  // per job: K, then delta_k
+    for (int j = 0; j < n_jobs; j++) {
+        const abg_profile_job& J = jobs[j];
+        char who[48];
+        snprintf(who, sizeof(who), "abg_history_profile: jobs[%d]", j);
+        const HiDev* h = monitor_dev(e, e->history, J.dev, who);
+        if (!h) return ABG_ERANGE;
+        const Device& d = e->dev[J.dev];
+        int rc = subband_check(who, d, e->B * d.hop, J.offset_hz, J.decim, J.n_coeffs, J.coeffs);
+        if (rc != ABG_OK) return rc;
+        if (J.n_tones < 0 || J.n_tones > ABG_TONE_MAX)
+            return fail(ABG_EINVAL, "%s: %d tones outside [0, %d]", who, J.n_tones, ABG_TONE_MAX);
+        const bool custom = J.tones && J.n_tones > 0;
+        const int K = custom ? J.n_tones : 51;
+        if ((rc = profile_shape_check(who, J.n_out, J.n_coeffs, K)) != ABG_OK) return rc;
+        if (!J.out) return fail(ABG_EINVAL, "%s: null out", who);
+        const double fs_out = (double)d.sample_rate / J.decim;
+        uint32_t* td = &tdelta[(size_t)j * (ABG_TONE_MAX + 1)];
+        td[0] = (uint32_t)K;
+        for (int k = 0; k < K; k++) {
+            const float f = custom ? J.tones[k] : kStandardTones[k];
+            if (!std::isfinite(f) || !(f > 0.0f) || !((double)f < fs_out / 2.0))
+                return fail(ABG_EINVAL, "%s: tone %d (%g Hz) outside (0, %g) Hz", who, k, (double)f, fs_out / 2.0);
+            td[1 + k] = (uint32_t)(unsigned long long)llround((double)f / fs_out * 4294967296.0);
+        }
+        // every tap in the history, abg_history_subband's rule: first_m D - (L - 1) >= first and (first_m + n - 1) D < end
+        const unsigned __int128 D = (unsigned)J.decim, lo = (unsigned __int128)J.first_m * D,
+                                hi = ((unsigned __int128)J.first_m + (unsigned long long)J.n_out - 1) * D;
+        if (h->first == h->end || lo < (unsigned __int128)h->first + (J.n_coeffs - 1) || hi >= h->end) {
+            const unsigned long long need_lo = (unsigned long long)(lo - std::min<unsigned __int128>(lo, J.n_coeffs - 1));
+            return fail(ABG_ERANGE, "%s: outputs [%llu, +%lld) at decimation %d with %d coefficients read samples [%llu, %llu], outside the history [%llu, %llu) of device %d",
+                        who, (unsigned long long)J.first_m, (long long)J.n_out, J.decim, J.n_coeffs, need_lo, (unsigned long long)hi,
+                        (unsigned long long)h->first, (unsigned long long)h->end, J.dev);
+        }
+        shapes[j] = ProfShape{J.first_m, J.n_out, J.n_coeffs, K};
+    }
+    std::vector<ProfPiece> ps;
+    std::vector<ProfPlanned> bs;
+    profile_plan(shapes, ps, bs);
+
+    auto& P = e->profile;
+    cudaSetDevice(e->cuda_dev);
+    if (!P.ev[0]) {
+        if (P.scratch.alloc(kProfileScratch) || P.res.alloc(kProfileResult)) {
+            P.scratch.free();
+            P.res.free();
+            return fail(ABG_ENOMEM, "Out of device memory for the transmission profile scratch");
+        }
+        if (cudaHostAlloc((void**)&P.h_res, sizeof(float) * kProfileResult, cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            P.h_res = nullptr;
+            P.scratch.free();
+            P.res.free();
+            return fail(ABG_ENOMEM, "Out of page-locked host memory for the transmission profile results");
+        }
+        for (auto& ev : P.ev) CU(cudaEventCreate(&ev));
+    }
+    P.ms[0] = P.ms[1] = 0.0f;
+    // per job: the sums in double, added block by block in block order
+    std::vector<abg_profile> acc(n_jobs);
+    memset(acc.data(), 0, sizeof(abg_profile) * n_jobs);
+    for (size_t p0 = 0, b0 = 0; p0 < ps.size();) {
+        size_t p1 = p0, b1 = b0;
+        while (p1 < ps.size() && ps[p1].chunk == ps[p0].chunk) p1++;
+        while (b1 < bs.size() && bs[b1].chunk == ps[p0].chunk) b1++;
+        const int rc = profile_chunk(e, jobs, tdelta, ps, p0, p1, bs, b0, b1);
+        if (rc != ABG_OK) return rc;
+        for (size_t i = b0; i < b1; i++) {
+            const ProfBlock& b = bs[i].b;
+            const float* r = P.h_res + b.res;
+            abg_profile& o = acc[bs[i].job];
+            o.p1 += r[0]; o.p2 += r[1]; o.a1 += r[2]; o.z[0] += r[3]; o.z[1] += r[4]; o.f1 += r[5]; o.f2 += r[6];
+            for (int k = 0; k < b.K; k++) {
+                o.tone_fm[k][0] += r[ABG_PROFILE_SUMS + 2 * k];
+                o.tone_fm[k][1] += r[ABG_PROFILE_SUMS + 2 * k + 1];
+                o.tone_am[k][0] += r[ABG_PROFILE_SUMS + 2 * b.K + 2 * k];
+                o.tone_am[k][1] += r[ABG_PROFILE_SUMS + 2 * b.K + 2 * k + 1];
+            }
+        }
+        p0 = p1;
+        b0 = b1;
+    }
+    for (int j = 0; j < n_jobs; j++) {
+        acc[j].n = jobs[j].n_out;
+        acc[j].n_tones = shapes[j].K;
+        memcpy(jobs[j].out, &acc[j], sizeof(abg_profile));
+    }
+    return ABG_OK;
+}
+
+int abg_debug_history_profile_time(abg_engine* e, float* ms2) {
+    if (!ms2) return fail(ABG_EINVAL, "abg_debug_history_profile_time: null argument");
+    memcpy(ms2, e->profile.ms, sizeof(e->profile.ms));
     return ABG_OK;
 }
 

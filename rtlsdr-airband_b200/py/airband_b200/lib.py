@@ -6,6 +6,7 @@ construction raises.  (The CPU oracle under oracle/ is test infrastructure and i
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import os
 from typing import List, Optional, Sequence, Tuple
 
@@ -34,12 +35,14 @@ SYMBOLS = [
     "abg_follow_open", "abg_follow_close", "abg_follow_run", "abg_follow_fetch", "abg_follow_info", "abg_follow_stats",
     "abg_debug_follow_time",
     "abg_history_spectrogram", "abg_history_activity", "abg_debug_history_analysis_time",
+    "abg_history_profile", "abg_debug_history_profile_time", "abg_debug_profile_plan",
 ]
 
 SUBBAND_MAX = 8            # ABG_SUBBAND_MAX: sub-band outputs per device
 SUBBAND_MAX_COEFFS = 4096  # ABG_SUBBAND_MAX_COEFFS
 TONE_MAX = 64              # ABG_TONE_MAX: tones in the tone meter's list
 ACTIVITY_MAX_RECORDS = 4096  # ABG_ACTIVITY_MAX_RECORDS: pieces one activity reading stores
+PROFILE_BLOCK = 1024       # ABG_PROFILE_BLOCK: outputs per block of a transmission profile
 BURST_OPEN_START, BURST_OPEN_END = 1, 2  # ABG_BURST_OPEN_START / ABG_BURST_OPEN_END
 # the tone meter's default list: the reference's standard CTCSS tones (CTCSS::standard_tones, src/ctcss.cpp:87-89)
 STANDARD_TONES = (67.0, 69.3, 71.9, 74.4, 77.0, 79.7, 82.5, 85.4, 88.5, 91.5, 94.8, 97.4, 100.0, 103.5, 107.2, 110.9, 114.8,
@@ -142,6 +145,39 @@ class CActivityJob(C.Structure):
         ("out", C.c_void_p),
         ("n_bursts", C.c_int32),
         ("n_truncated", C.c_int32),
+    ]
+
+
+class CProfile(C.Structure):
+    """abg_profile: the sums of one transmission profile (definition in airband_b200.h)."""
+    _fields_ = [
+        ("n", C.c_int64),
+        ("n_tones", C.c_int32),
+        ("reserved", C.c_int32),
+        ("p1", C.c_double),
+        ("p2", C.c_double),
+        ("a1", C.c_double),
+        ("z", C.c_double * 2),
+        ("f1", C.c_double),
+        ("f2", C.c_double),
+        ("tone_fm", (C.c_double * 2) * TONE_MAX),
+        ("tone_am", (C.c_double * 2) * TONE_MAX),
+    ]
+
+
+class CProfileJob(C.Structure):
+    """abg_profile_job: one transmission profile job (definition in airband_b200.h)."""
+    _fields_ = [
+        ("dev", C.c_int32),
+        ("decim", C.c_int32),
+        ("offset_hz", C.c_double),
+        ("n_coeffs", C.c_int32),
+        ("n_tones", C.c_int32),
+        ("coeffs", C.c_void_p),
+        ("first_m", C.c_uint64),
+        ("n_out", C.c_int64),
+        ("tones", C.c_void_p),
+        ("out", C.POINTER(CProfile)),
     ]
 
 
@@ -252,6 +288,10 @@ def load():
     L.abg_history_spectrogram.restype, L.abg_history_spectrogram.argtypes = i, [vp, i, C.POINTER(CSpectrogramJob)]
     L.abg_history_activity.restype, L.abg_history_activity.argtypes = i, [vp, i, C.POINTER(CActivityJob)]
     L.abg_debug_history_analysis_time.restype, L.abg_debug_history_analysis_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_history_profile.restype, L.abg_history_profile.argtypes = i, [vp, i, C.POINTER(CProfileJob)]
+    L.abg_debug_history_profile_time.restype, L.abg_debug_history_profile_time.argtypes = i, [vp, C.POINTER(C.c_float)]
+    L.abg_debug_profile_plan.restype = i
+    L.abg_debug_profile_plan.argtypes = [i, vp, vp, vp, vp, vp, vp, i, C.POINTER(C.c_int32), vp, i, C.POINTER(C.c_int32)]
     L.abg_debug_tc_table.restype = i
     L.abg_debug_tc_table.argtypes = [i, i, i, f, i, vp, i, vp, vp, C.c_size_t, vp, C.POINTER(C.c_double)]
     _LIB = L
@@ -743,6 +783,37 @@ class Engine:
         self._chk(self.L.abg_debug_history_analysis_time(self.h, ms))
         return float(ms[0]), float(ms[1]), float(ms[2])
 
+    # ---- transmission profiles ------------------------------------------------------------------------------------
+    def history_profile(self, jobs) -> List[dict]:
+        """The profile sums of windows of the history, all jobs in one call (definition in airband_b200.h).  jobs: dicts
+        with dev, offset_hz, decim, coeffs, first_m, n_out and tones (None: the 51 standard tones), e.g. from profile_job.
+        Returns per job a dict: n, p1, p2, a1, z (complex), f1, f2, tone_fm and tone_am (complex128[K])."""
+        arr = (CProfileJob * max(len(jobs), 1))()
+        outs = (CProfile * max(len(jobs), 1))()
+        keep = []
+        for k, j in enumerate(jobs):
+            h = np.ascontiguousarray(j["coeffs"], dtype=np.float32)
+            t = j.get("tones")
+            t = np.ascontiguousarray(t, dtype=np.float32) if t is not None and len(t) else None
+            keep.append((h, t))
+            arr[k] = CProfileJob(int(j["dev"]), int(j["decim"]), float(j["offset_hz"]), h.size, 0 if t is None else t.size, _ptr(h),
+                                 int(j["first_m"]), int(j["n_out"]), _ptr(t), C.pointer(outs[k]))
+        self._chk(self.L.abg_history_profile(self.h, len(jobs), arr))
+        res = []
+        for k in range(len(jobs)):
+            o, K = outs[k], outs[k].n_tones
+            fm, am = np.ctypeslib.as_array(o.tone_fm)[:K], np.ctypeslib.as_array(o.tone_am)[:K]
+            res.append(dict(n=int(o.n), p1=o.p1, p2=o.p2, a1=o.a1, z=complex(o.z[0], o.z[1]), f1=o.f1, f2=o.f2,
+                            tone_fm=fm[:, 0] + 1j * fm[:, 1], tone_am=am[:, 0] + 1j * am[:, 1]))
+        return res
+
+    def history_profile_time(self) -> Tuple[float, float]:
+        """(capture ms, profile kernel ms) of the most recent history_profile, summed over its chunks, from CUDA events;
+        0 before the first."""
+        ms = (C.c_float * 2)()
+        self._chk(self.L.abg_debug_history_profile_time(self.h, ms))
+        return float(ms[0]), float(ms[1])
+
     # ---- mixers ---------------------------------------------------------------------------------------------------
     def configure_mixers(self, mixers: Sequence[Sequence[Tuple[int, int, float, float]]]) -> None:
         """mixers[m] = [(dev, chan, ampfactor, balance), ...]"""
@@ -1230,3 +1301,171 @@ def history_transmissions(e: Engine, cfg: Config, dev: int, margin_db: float, ha
     thr = activity_threshold(spec, margin_db, half_width)
     act = e.history_activity([dict(dev=dev, first_batch=b0, n_batches=nb, stride=stride, hang=hang, min_span=min_span, thr=thr)])[0]
     return group_transmissions(act["bursts"], cfg, dev, max_bin_gap=max_bin_gap)
+
+
+# ---- transmission profiles ----------------------------------------------------------------------------------------------
+def profile_plan(first_m, n_out, n_coeffs, n_tones):
+    """Host-only: the chunk and block plan abg_history_profile launches for jobs of these shapes (abg_debug_profile_plan).
+    Returns (limits dict, pieces int64[P, 6], blocks int64[Q, 8]); the columns are named in airband_b200.h."""
+    L = load()
+    fm = np.ascontiguousarray(first_m, np.uint64)
+    n = np.ascontiguousarray(n_out, np.int64)
+    lc = np.ascontiguousarray(n_coeffs, np.int32)
+    k = np.ascontiguousarray(n_tones, np.int32)
+    lim = np.zeros(4, np.int64)
+    npc, nbk = C.c_int32(0), C.c_int32(0)
+    args = lambda p, cp, b, cb: (fm.size, _ptr(fm), _ptr(n), _ptr(lc), _ptr(k), _ptr(lim), _ptr(p), cp, C.byref(npc), _ptr(b), cb, C.byref(nbk))  # noqa: E731
+    rc = L.abg_debug_profile_plan(*args(None, 0, None, 0))
+    if rc < 0:
+        raise AbgError(rc, (L.abg_last_error() or b"").decode())
+    pieces, blocks = np.zeros((npc.value, 6), np.int64), np.zeros((nbk.value, 8), np.int64)
+    L.abg_debug_profile_plan(*args(pieces, pieces.shape[0], blocks, blocks.shape[0]))
+    return dict(scratch=int(lim[0]), blocks=int(lim[1]), result=int(lim[2]), coeffs=int(lim[3])), pieces, blocks
+
+
+# The default down-converter of a profile job.  Its passband has to hold an NFM signal of 5 kHz deviation with 3 kHz audio
+# (Carson: 8 kHz each side) wherever the transmission's frequency puts it: group_transmissions' frequency is good to about
+# one bin, sample_rate // fft_size.  So the cutoff is 8 kHz + one bin, and the Kaiser filter's 60 dB stopband starts at
+# twice the cutoff: L = ceil((60 - 7.95) / (14.36 cutoff) * sample_rate) + 1, odd.  The decimation makes the output noise
+# white: D is the integer in [0.8, 1.2] * sample_rate / (2 cutoff) where the filter's autocorrelation at lag D (the output
+# noise's lag-1 correlation rho) is smallest.  That keeps the noise's own real lag-1 term rho sigma^2 out of z, which
+# otherwise pulls arg(z) towards the down-converter's frequency (12 Hz at a 2 kHz offset and 20 dB with rho = 0.6), and
+# needs no estimate of sigma^2, which a deep AM envelope spoils.  It lands at fs_out ~ 1.77 cutoff; the largest
+# instantaneous frequency, one bin + 5 kHz, stays below fs_out / 2.  At 2.048 and 2.56 Msps and fft 512 to 8192 that is
+# cutoff 8.25 - 13 kHz, fs_out 14.6 - 23 kHz, L 621 - 1119 and |rho| < 0.004.
+PROFILE_SWING_HZ = 8000.0
+
+
+def profile_filter(cfg: Config, dev: int) -> Tuple[int, float, int]:
+    """(decim, cutoff_hz, n_coeffs) of the default profile down-converter of device dev (the rule above)."""
+    return _profile_filter(int(cfg.devices[dev].sample_rate), int(cfg.fft_size))[:3]
+
+
+@functools.lru_cache(maxsize=64)
+def _profile_filter(sr: int, fft_size: int):
+    """(D, cutoff, L, h) of the rule above; the search over D costs about a millisecond, so it is done once per shape."""
+    cutoff = PROFILE_SWING_HZ + sr // fft_size
+    L = min((int(np.ceil((60.0 - 7.95) / (14.36 * cutoff) * sr)) + 1) | 1, SUBBAND_MAX_COEFFS - 1)
+    h = subband_lowpass(L, cutoff, sr).astype(np.float64)
+    e = float(np.dot(h, h))
+    d0 = sr / (2.0 * cutoff)
+    cand = range(max(1, int(0.8 * d0)), max(1, int(1.2 * d0)) + 1)
+    D = min(cand, key=lambda D: abs(float(np.dot(h[D:], h[:-D])) / e) if D < L else 0.0)
+    return int(D), float(cutoff), L, h.astype(np.float32)
+
+
+def profile_job(tx: dict, cfg: Config, dev: int, history_range: Tuple[int, int], decim: Optional[int] = None,
+                cutoff_hz: Optional[float] = None, n_coeffs: Optional[int] = None, tones: Optional[Sequence[float]] = None) -> dict:
+    """An Engine.history_profile job for one transmission (a group_transmissions dict of device dev): the down-converter
+    at tx["freq_hz"] (defaults from profile_filter, coefficients from subband_lowpass) over the transmission's samples
+    [first_frame * hop, last_frame * hop + fft_size), as the outputs m with m * decim inside them, clipped so that every
+    tap lies in history_range (transmission_capture's window).  tones None: the 51 standard tones.  Raises ValueError
+    if fewer than 2 outputs are left."""
+    D0, c0, L0 = profile_filter(cfg, dev)
+    D = D0 if decim is None else int(decim)
+    cutoff = c0 if cutoff_hz is None else float(cutoff_hz)
+    L = L0 if n_coeffs is None else int(n_coeffs)
+    off, m0, n = transmission_capture(tx, cfg, dev, history_range, D, L)
+    if n < 2:
+        raise ValueError(f"profile_job: {n} output of the transmission fits the history (at least 2)")
+    if (D, cutoff, L) == (D0, c0, L0):
+        h = _profile_filter(int(cfg.devices[dev].sample_rate), int(cfg.fft_size))[3].copy()
+    else:
+        h = subband_lowpass(L, min(cutoff, cfg.devices[dev].sample_rate / 2), cfg.devices[dev].sample_rate)
+    return dict(dev=dev, offset_hz=off, decim=D, coeffs=h, first_m=m0, n_out=n, tones=list(tones) if tones is not None and len(tones) else None)
+
+
+# The decision rule (DESIGN §4, "Transmission profiles", gives its calibration).  With the output noise's lag-1
+# correlation rho (the filter's autocorrelation at lag D over its energy), u = var(a) / mean(a)^2 and w = var(phi):
+# circular noise adds sigma^2 / 2C to u and (1 - rho) sigma^2 / C to w, so an AM envelope shows as d = u - w / (2 (1 - rho))
+# > 0 and FM as d < 0, the noise cancelling.  Below about 15 dB the phase noise is no longer Gaussian (clicks) and d loses
+# its sign, so the rule decides only when the SNR estimate, the larger of the two hypotheses' own estimates (from the
+# envelope's kurtosis for a constant envelope, from w for a constant phase), is at least PROFILE_MIN_SNR_DB.
+PROFILE_MIN_SNR_DB = 15.0
+PROFILE_AM_MIN_D = -0.006       # d above it: AM (a bare carrier reads d ~ 0)
+PROFILE_AM_SURE_D = 0.04        # d above it: AM at any SNR (nothing else reads above -0.006 at 10 dB)
+PROFILE_NOISE_KAPPA = 0.9       # envelope spread of noise alone: 1
+PROFILE_CTCSS_MIN_SHARE = 0.005  # ctcss_identify's share rule
+PROFILE_CTCSS_MIN_S = 0.4        # the reference's CTCSS window
+
+
+def _tone_basis(m0: int, count: int, tones, fs_out: float) -> np.ndarray:
+    """sum_{m0 <= m < m0 + count} exp(-2 pi i (delta_k m mod 2^32) / 2^32) per tone, in double (a geometric series)."""
+    d = np.array([int(np.floor(float(np.float32(f)) / fs_out * 4294967296.0 + 0.5)) % (1 << 32) for f in tones], np.float64)
+    w = -2.0 * np.pi * d / 4294967296.0
+    out = np.empty(len(d), np.complex128)
+    for k, wk in enumerate(w):
+        r = np.exp(1j * wk)
+        out[k] = count if abs(1 - r) < 1e-15 else np.exp(1j * ((int(d[k]) * (m0 % (1 << 32))) % (1 << 32)) * -2.0 * np.pi / 4294967296.0) * (1 - r ** count) / (1 - r)
+    return out
+
+
+def profile_summary(reading: dict, job: dict, cfg: Config, dev: int) -> dict:
+    """What a profile reading (Engine.history_profile) says of its transmission: freq_hz (absolute: centre +
+    subband_frequency(offset) + the measured offset, from arg(z) for AM and from f1 / (n - 1) for NFM), modulation
+    (config.MOD_AM, MOD_NFM or None when undecided; a bare carrier counts as AM), am_depth, fm_deviation_hz (peak, for a
+    sinusoidal modulation), snr_db, ctcss_hz and ctcss_share (the strongest tone of the decided modulation's tone sums by
+    tone_powers' share, after removing the mean's own leakage; None below PROFILE_CTCSS_MIN_SHARE or for windows under
+    PROFILE_CTCSS_MIN_S), and channel_kw = dict(modulation=..., ctcss_hz=...) for transmission_replay (ctcss_hz 0.0 for
+    no tone, as make_channel takes it; an undecided profile's modulation is None, which make_channel refuses)."""
+    from .config import MOD_AM, MOD_NFM
+    d = cfg.devices[dev]
+    D = int(job["decim"])
+    fs_out = d.sample_rate / D
+    h = np.asarray(job["coeffs"], np.float64)
+    rho = float(np.dot(h[D:], h[:-D]) / np.dot(h, h)) if D < h.size else 0.0
+    n = int(reading["n"])
+    npair = n - 1
+    mean_a = reading["a1"] / n
+    u = max(reading["p1"] / n - mean_a ** 2, 0.0) / mean_a ** 2 if mean_a > 0 else 1.0
+    mean_phi = reading["f1"] / npair
+    w = max(reading["f2"] / npair - mean_phi ** 2, 0.0)
+    kappa = n * reading["p2"] / reading["p1"] ** 2 - 1.0 if reading["p1"] > 0 else 1.0
+    s_fm = ((1 - kappa) + np.sqrt(1 - kappa)) / kappa if 0 < kappa < 1 else (np.inf if kappa <= 0 else 0.0)
+    s_am = (1 - rho) / w if w > 0 else np.inf
+    snr = max(s_fm, s_am)
+    snr_db = float(10 * np.log10(snr)) if snr > 0 else -np.inf
+    dstat = u - w / (2 * (1 - rho))
+    mod = None
+    if snr_db >= PROFILE_MIN_SNR_DB:
+        mod = MOD_AM if dstat > PROFILE_AM_MIN_D else MOD_NFM
+    elif dstat > PROFILE_AM_SURE_D and kappa < PROFILE_NOISE_KAPPA:  # deep AM: its troughs spoil both SNR estimates
+        mod = MOD_AM
+    if mod == MOD_NFM:
+        off = mean_phi * fs_out / (2 * np.pi)
+    else:  # the noise's own lag-1 correlation, rho sigma^2 per pair, is real and pulls arg(z) towards 0; profile_filter's
+        # D makes rho ~ 0, and for other filters sigma^2 = P / (1 + s) removes it to first order
+        sigma2 = reading["p1"] / n / (1.0 + s_am) if np.isfinite(s_am) and snr_db >= PROFILE_MIN_SNR_DB else 0.0
+        off = float(np.angle(reading["z"] - rho * sigma2 * npair)) * fs_out / (2 * np.pi)
+    freq = float(d.centerfreq) + subband_frequency(job["offset_hz"], d.sample_rate) + off
+    tones = job.get("tones")
+    tones = tuple(tones) if tones is not None and len(tones) else STANDARD_TONES  # [] or None: the standard tones, as the call takes them
+    ctcss = share = None
+    if mod is not None and n / fs_out >= PROFILE_CTCSS_MIN_S:
+        if mod == MOD_NFM:
+            S = reading["tone_fm"] - mean_phi * _tone_basis(job["first_m"], npair, tones, fs_out)
+            cnt, E = npair, npair * w
+        else:
+            S = reading["tone_am"] - mean_a * _tone_basis(job["first_m"], n, tones, fs_out)
+            cnt, E = n, n * u * mean_a ** 2
+        sh = 2.0 * np.abs(S) ** 2 / (cnt * E) if E > 0 else np.zeros(len(tones))
+        k = int(np.argmax(sh))
+        if sh[k] >= PROFILE_CTCSS_MIN_SHARE:
+            ctcss, share = float(tones[k]), float(sh[k])
+    return dict(freq_hz=freq, modulation=mod, snr_db=snr_db,
+                am_depth=float(np.sqrt(2 * max(dstat, 0.0))) if mod == MOD_AM else None,
+                fm_deviation_hz=float(np.sqrt(2 * max(w - 2 * (1 - rho) * u, 0.0)) * fs_out / (2 * np.pi)) if mod == MOD_NFM else None,
+                ctcss_hz=ctcss, ctcss_share=share, channel_kw=dict(modulation=mod, ctcss_hz=ctcss or 0.0))
+
+
+def history_profiles(e: Engine, cfg: Config, dev: int, txs, **job_kw) -> List[dict]:
+    """profile_summary of every transmission of device dev (group_transmissions dicts, e.g. from history_transmissions),
+    measured in one Engine.history_profile call; job_kw goes to profile_job.  Each summary also holds its job.  The
+    result plugs into transmission_replay: transmission_replay(dict(tx, freq_hz=s["freq_hz"]), cfg, dev, hist,
+    **s["channel_kw"])."""
+    hist = e.history_range(dev)
+    jobs = [profile_job(tx, cfg, dev, hist, **job_kw) for tx in txs]
+    if not jobs:
+        return []
+    readings = e.history_profile(jobs)
+    return [dict(profile_summary(r, j, cfg, dev), job=j) for r, j in zip(readings, jobs)]
